@@ -37,11 +37,11 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "vSLAM frames/s (AKAZE+match+RANSAC, 1080p ~5k kp) at 1/2/4/8 B200"     # BASELINE.json, verbatim
+METRIC = "vSLAM frames/s (AKAZE+match+RANSAC, 1080p ~5k kp) at 1/2/4/8 H100"     # BASELINE.json, verbatim
 W, H = 1920, 1080
 MAXF = 5000            # maximum_features -> exactly "~5k keypoints" per frame
 BETTER_BY = 24         # cv-sfm/src/settings.rs:397-399
-POOL_PAIRS = 8         # 16 distinct frames = 133 MB > 126 MB L2: step inputs are never L2-resident
+POOL_PAIRS = 8         # 16 distinct frames = 133 MB > 50 MB L2: step inputs are never L2-resident
 PAIRS_PER_STEP = 16    # one step = one batch of 16 frame pairs (32 frames)
 FOCAL, CX, CY = 1000.0, 960.0, 540.0
 ARRSAC = dict(threshold=1e-7, initialization_hypotheses=8192, max_candidate_hypotheses=1024)      # vslam-sandbox/src/main.rs:112-117
@@ -269,6 +269,40 @@ def track256(rank, world, ctxs):
             "timing": "host API (host pointers in, results on the host), wall clock, this rank's replica"}
 
 
+def write_outputs(out_dir, results, pool_index, cap):
+    """--dump-outputs: the results of the last timed step's frame pairs (in pair order) as .npy files, ~47 MB in all.  Rows past a
+    pair's count are zero (keypoints, descriptors) or -1 (matches, inliers).  Keypoints, descriptors and matches depend only on
+    the frames, and the consensus (pose, inliers) also on the pair's index, which seeds its generator.  A pair without a model has a
+    zero pose and no inliers."""
+    from cv_b200._lib import KP_DTYPE
+    os.makedirs(out_dir, exist_ok=True)
+    P = len(results)
+    kps = np.zeros((P, 2, cap, len(KP_DTYPE.names)), np.float32)
+    desc = np.zeros((P, 2, cap, 64), np.float32)
+    nkp = np.zeros((P, 2), np.float32)
+    matches = np.full((P, cap, 2), -1.0, np.float32)
+    inliers = np.full((P, cap), -1.0, np.float32)
+    counts = np.zeros((P, 3), np.float32)          # matches, inliers, found
+    pose = np.zeros((P, 12), np.float64)           # R (row-major) then t
+    for p, (n, kp, d, cnt, pairs, model, inl) in enumerate(results):
+        kp = kp.view(KP_DTYPE).reshape(2, cap)
+        for f in range(2):
+            k = int(n[f])
+            nkp[p, f] = k
+            kps[p, f, :k] = np.stack([kp[f][name][:k].astype(np.float32) for name in KP_DTYPE.names], 1)
+            desc[p, f, :k] = d.reshape(2, cap, 64)[f, :k]
+        npairs, ninl, found = int(cnt[0]), int(cnt[1]), int(cnt[2]) == 1
+        counts[p] = [npairs, ninl if found else 0, found]
+        matches[p, :npairs] = pairs.reshape(cap, 2)[:npairs]
+        if found:
+            inliers[p, :ninl] = inl[:ninl]
+            pose[p] = model
+    arrays = {"keypoints": kps, "keypoint_counts": nkp, "descriptors": desc, "matches": matches, "inliers": inliers,
+              "match_inlier_found_counts": counts, "pose": pose, "frame_pool_index": np.asarray(pool_index, np.float32)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def bind_to_gpu_numa_node(props):
     """Run this process (and the pinned buffers it first-touches) on the CPUs local to the GPU's PCIe root, like a deployed
     service would; silently skipped when sysfs does not expose the topology."""
@@ -292,6 +326,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="cvb200")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned to its caller as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -333,8 +369,8 @@ def main():
     h_pool = [torch.from_numpy(p).pin_memory() for p in frames]
 
     class Slot:
-        """Everything one context owns: device result buffers, pinned host result buffers, its consensus generator (the
-        two_view_consensus object of a VSlam instance keeps its generator across frame pairs)."""
+        """Everything one context owns: device result buffers, pinned host result buffers, the consensus generator of the pair it
+        runs (seeded from the pair's index in the frame stream, so a pair's result does not depend on which context ran it)."""
         def __init__(self):
             self.kp = torch.empty(2 * cap * KP_DTYPE.itemsize, dtype=torch.uint8, device=dev)
             self.desc = torch.zeros(2 * cap * 64, dtype=torch.uint8, device=dev)
@@ -351,16 +387,19 @@ def main():
             self.h_np, self.h_ni, self.h_found = C.c_uint32(), C.c_uint32(), C.c_int32()
             self.h_model = Pose()
             self.rng = Rng()
-            lib.cvb_rng_seed_xoshiro256pp(C.byref(self.rng), 0)
             self.stats = (C.c_uint32 * 16)()
             self.pairs_done = 0
             self.t_busy = 0.0
     slots = [Slot() for _ in range(NCTX)]
 
+    dump_first = (Wm + K - 1) * PAIRS_PER_STEP if args.dump_outputs and rank == 0 else None     # first pair of the last timed step
+    dumped = {}
+
     def pair_dev(i, c):
         """device-resident: frames already in HBM, results stay in HBM; one synchronisation (the generator commit)"""
         cx, s = ctxs[c], slots[c]
         img = d_pool[i % POOL_PAIRS]
+        lib.cvb_rng_seed_xoshiro256pp(C.byref(s.rng), i)
         cx.check(lib.cvb_akaze_extract_batch_dev(cx.handle, C.byref(akaze_cfg), img.data_ptr(), 2, W, H, s.kp.data_ptr(), s.desc.data_ptr(), cap,
                                                  s.n.data_ptr()))
         cx.check(lib.cvb_two_view_pair_dev(cx.handle, s.kp.data_ptr(), s.desc.data_ptr(), s.n.data_ptr(),
@@ -368,11 +407,14 @@ def main():
                                            BETTER_BY, C.byref(intr), C.addressof(acfg), C.addressof(s.rng), s.pairs.data_ptr(), cap,
                                            s.cnt.data_ptr(), s.model.data_ptr(), s.inl.data_ptr(), s.cnt.data_ptr() + 4, s.cnt.data_ptr() + 8))
         cx.check(lib.cvb_arrsac_commit_rng(cx.handle, C.addressof(s.rng), s.stats))
+        if dump_first is not None and i >= dump_first:      # the stream is drained: copy this pair's results before the slot is reused
+            dumped[i] = [t.cpu().numpy() for t in (s.n, s.kp, s.desc, s.cnt, s.pairs, s.model, s.inl)]
 
     def pair_host(i, c):
         """end to end: pinned host frames in, every result back on the host"""
         cx, s = ctxs[c], slots[c]
         img = h_pool[i % POOL_PAIRS]
+        lib.cvb_rng_seed_xoshiro256pp(C.byref(s.rng), i)
         cx.check(lib.cvb_two_view_frames(cx.handle, C.addressof(akaze_cfg), img.data_ptr(), W, H, BETTER_BY, C.byref(intr), C.addressof(acfg),
                                          C.addressof(s.rng), s.h_kp.data_ptr(), s.h_desc.data_ptr(), cap, s.h_n, s.h_pairs.data_ptr(),
                                          C.byref(s.h_np), C.byref(s.h_model), s.h_inl.data_ptr(), C.byref(s.h_ni), C.byref(s.h_found)))
@@ -406,9 +448,8 @@ def main():
             dist.barrier()
             torch.cuda.synchronize()
 
-    def reset_rngs():
+    def reset_counters():
         for s in slots:
-            lib.cvb_rng_seed_xoshiro256pp(C.byref(s.rng), 0)
             s.pairs_done = 0; s.t_busy = 0.0
 
     # ---- setup (not a warm-up step): every (context, input buffer) pair captures its extraction graph; workspaces are allocated
@@ -425,7 +466,7 @@ def main():
     sampler.start()
 
     # ---- value: device-resident, W warm-up steps then exactly K timed steps of PAIRS_PER_STEP pairs
-    reset_rngs()
+    reset_counters()
     run_pairs(pair_dev, 0, Wm * PAIRS_PER_STEP)
     barrier()
     l0 = sum(cx.launch_count() for cx in ctxs)
@@ -447,7 +488,7 @@ def main():
     cnt0 = slots[0].cnt.cpu().numpy().tolist()
 
     # ---- e2e: host entry point, pinned host buffers, copies inside the timed region
-    reset_rngs()
+    reset_counters()
     run_pairs(pair_host, 0, Wm * PAIRS_PER_STEP)
     barrier()
     for s in slots:
@@ -474,6 +515,8 @@ def main():
     per_rank_all = [[round(float(v), 3) for v in t.cpu().tolist()] for t in per_rank_all]
     e2e_busy = [round(s.t_busy / max(s.pairs_done, 1) * 1e3, 3) for s in slots]
     e2e_pairs = [s.pairs_done for s in slots]
+    if dump_first is not None:
+        write_outputs(args.dump_outputs, [dumped[i] for i in sorted(dumped)], [i % POOL_PAIRS for i in sorted(dumped)], cap)
     sampler.stop_flag = True
     sampler.join(timeout=2)
 
@@ -482,7 +525,6 @@ def main():
     ransac = None
     if rank == 0:
         try:
-            lib.cvb_rng_seed_xoshiro256pp(C.byref(s0.rng), 0)
             pair_host(0, 0)
             npairs, ninl = int(s0.h_np.value), int(s0.h_ni.value)
             kp = np.frombuffer(s0.h_kp.numpy().tobytes(), dtype=KP_DTYPE)
@@ -538,7 +580,6 @@ def main():
     # ---- roofline: instrumented pass (per-kernel CUDA events on the launching stream, one context, no overlap)
     ctx.profile(True)
     PK = 6
-    lib.cvb_rng_seed_xoshiro256pp(C.byref(slots[0].rng), 0)
     for i in range(PK):
         pair_dev(i, 0)
     rep = ctx.profile_report()
@@ -548,8 +589,8 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s"
     tot_ms = sum(v["ms"] for v in rep.values())
     top = max(rep.items(), key=lambda kv: kv[1]["ms"]) if rep else (None, None)
     kernels = {k: {"launches_per_pair": v["launches"] / PK, "ms_per_pair": v["ms"] / PK, "share": v["ms"] / tot_ms if tot_ms else 0,
@@ -557,16 +598,9 @@ def main():
     hb = {k: v for k, v in rep.items() if v["bytes"] > 0 and k != "k_hamming_knn"}      # the matcher's 64 B/cmp is a streaming model, not traffic
     dom = max(hb.items(), key=lambda kv: kv[1]["ms"])
     achieved = dom[1]["bytes"] / (dom[1]["ms"] * 1e-3) / 1e9
-    traffic, traffic_src = None, None
-    try:      # DRAM bytes per launch of the dominant kernel from the committed ncu capture (profiles/), not measured live
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get(dom[0])
-        if tj:
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
-    except Exception:
-        pass
     fps_rank = value / world
     roofline = {"bound": "hbm", "kernel": dom[0], "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "launch_ms": dom[1]["ms"] / dom[1]["launches"], "bytes_per_launch": dom[1]["bytes"] / dom[1]["launches"],
                 "timing": "per-kernel CUDA events on the launching stream, separate instrumented pass of the same pairs (one context, no overlap)",
                 "pipeline_alg_GBps": fps_rank * ALG_BYTES_PER_FRAME / 1e9, "pipeline_frac": fps_rank * ALG_BYTES_PER_FRAME / 1e9 / hbm_peak,
@@ -597,9 +631,9 @@ def main():
                 "config": {"workload": WORKLOAD, "pairs_per_step": PAIRS_PER_STEP, "frames_per_step_per_gpu": 2 * PAIRS_PER_STEP,
                            "keypoints_per_frame": n_kp, "matches": cnt0[0], "inliers": cnt0[1], "maximum_features": MAXF,
                            "detector_threshold": 0.001, "better_by": BETTER_BY, "arrsac": ARRSAC, "intrinsics": [FOCAL, FOCAL, CX, CY],
-                           "pipelining": f"{NCTX} contexts (CUDA stream + workspace + host thread + consensus generator each) take pairs from a "
-                                         "shared queue; extraction is one CUDA graph per context",
-                           "l2": f"inputs rotate over a pool of {2 * POOL_PAIRS} distinct frames ({2 * POOL_PAIRS * W * H * 4 / 1e6:.0f} MB > 126 MB L2)",
+                           "pipelining": f"{NCTX} contexts (CUDA stream + workspace + host thread each) take pairs from a "
+                                         "shared queue; extraction is one CUDA graph per context; pair i's consensus generator is seeded with i",
+                           "l2": f"inputs rotate over a pool of {2 * POOL_PAIRS} distinct frames ({2 * POOL_PAIRS * W * H * 4 / 1e6:.0f} MB > 50 MB L2)",
                            "setup": "graph capture / allocation pass over every (context, input) pair before the warm-up steps"},
                 "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d_step, "d2h_bytes_per_step": d2h_step,
                         "host_threads": NCTX, "timed_region_ms": ms_e2e, "mean_call_ms": sum(e2e_busy) / len(e2e_busy),

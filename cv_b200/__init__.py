@@ -1,4 +1,4 @@
-"""cv_b200 -- B200-native (sm_100a) drop-in for rust-cv's AKAZE -> Hamming match -> RANSAC hot path.
+"""cv_b200 -- H100-native (sm_90a) drop-in for rust-cv's AKAZE -> Hamming match -> RANSAC hot path.
 
 Host-side mirror of the reference's interfaces for this path, over the C ABI in include/cvb200.h:
 
@@ -8,7 +8,7 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
 
 There is no CPU fallback: every call runs CUDA kernels from cv_b200/libcvb200.so and raises
-CvbError when the library or a Blackwell GPU is missing.
+CvbError when the library or a Hopper (sm_90) GPU is missing.
 """
 from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F401
 from .akaze import Akaze, AkazeConfig  # noqa: F401

@@ -116,7 +116,7 @@ class Context:
         h = C.c_void_p()
         rc = self.lib.cvb_ctx_create_on_stream(int(device), C.c_void_p(stream) if stream else None, C.byref(h))
         if rc != 0:
-            raise CvbError(rc, "cvb_ctx_create failed (a Blackwell-class CUDA device is required; there is no CPU fallback)")
+            raise CvbError(rc, "cvb_ctx_create failed (a Hopper (sm_90) CUDA device is required; there is no CPU fallback)")
         self.handle = h
         self.device = device
 

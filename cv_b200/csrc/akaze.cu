@@ -120,7 +120,7 @@ struct AkazeWorkspace {
     CUtensorMap *tmaps = nullptr;      // device: [3][MAX_EVO] per-evolution maps (deriv1 source, Lx, Ly) for the TMA-staged tiles
     bool use_tma = false;
     int tma_mask = 3;                  // CVB_TMA_MASK: 1 k_blur_v3, 2 k_blur_scharr_pm, 4 k_deriv1_v3, 8 k_deriv2_v3.  Default: the two blur kernels
-                                       // (measured on B200: blur -8 %, blur+Scharr -1 %, derivative kernels +25 % with the single-stage TMA path)
+                                       // (the single-stage TMA path stages wider boxes than the derivative kernels' classic path reads)
     SupScratch sup{};
     bool suppress_seq = false;   // CVB_SUPPRESS_SEQ=1: serial reference kernel (debug / A-B check)
     bool suppress_par_only = false;   // CVB_SUPPRESS_GLOBAL=1: force the global-memory parallel kernel

@@ -1,10 +1,10 @@
-// cv_b200/csrc/akaze_kernels.cuh -- sm_100a kernels of the AKAZE extractor.
+// cv_b200/csrc/akaze_kernels.cuh -- sm_90a kernels of the AKAZE extractor.
 //
 // Parity contract: every f32 value produced here is bit-identical to what rust-cv `akaze` 0.7.0
 // computes on a default x86-64 build (unfused multiply-add, wide::f32x4 lane sums reduced as
 // (l0+l2)+(l1+l3)).  Stages may be FUSED (intermediates live in shared memory, never in HBM) but
 // each intermediate is rounded to f32 exactly where the reference materialises it.
-// Compile with -fmad=false.  Reference line numbers are relative to /root/reference/akaze/src.
+// Compile with -fmad=false.  Reference line numbers are relative to the reference's akaze/src.
 #pragma once
 #include <cuda.h>            // CUtensorMap (types only: the encode entry point is resolved at run time, no libcuda link dependency)
 #include <cuda/barrier>      // cuda::barrier + the cp.async.bulk.tensor wrappers (libcu++, header only)
@@ -461,8 +461,8 @@ constexpr int SW3 = 32, SH3 = 64, STRIP = 8;
 // image is fetched by ONE 3-D cp.async.bulk.tensor (x, y, frame) issued by one thread and awaited on an mbarrier; tiles that touch the
 // border keep the clamped path below, because TMA fills out-of-bounds elements with zero while the reference replicates the border
 // (image.rs:233-235,289-296).  The box is `pitch3(R)` floats wide; the padding columns are never read.  Shared-memory contents of the halo region are identical in both paths.
-// The TMA unit faults ("illegal instruction") when a box starts at an x coordinate that is not a multiple of 16 bytes (measured on
-// B200: x = 64 loads, x = 190 faults, 2-D and 3-D alike), so the staged box starts xpad3(R) >= R floats left of the tile, a multiple of
+// A box that starts at an x coordinate that is not a multiple of 16 bytes faults ("illegal instruction"; x = 64 loads, x = 190 faults,
+// 2-D and 3-D alike, in a stand-alone probe), so the staged box starts xpad3(R) >= R floats left of the tile, a multiple of
 // 4 floats, and the kernels read their halo region at column offset xoff3(R) inside it.
 __host__ __device__ constexpr int xpad3(int r) { return r <= 4 ? 4 : 8; }
 __host__ __device__ constexpr int xoff3(int r) { return xpad3(r) - r; }
@@ -470,7 +470,7 @@ __host__ __device__ constexpr int pitch3(int r) { return SW3 + 2 * xpad3(r); }
 // The TMA path follows the CUDA programming guide's tensor-copy protocol through libcu++ (cuda::barrier in shared memory,
 // fence.proxy.async after its initialisation, every thread arrives, the issuing thread adds the transaction bytes): a hand-written
 // mbarrier.init / fence.mbarrier_init / expect_tx sequence that serves the 1-D bulk copies of the matcher raised "illegal
-// instruction" on UTMALDG on B200 (scratch probe), the guide's protocol does not.
+// instruction" on UTMALDG in a stand-alone probe, the guide's protocol does not.
 using ak_barrier = cuda::barrier<cuda::thread_scope_block>;
 
 template <int RX, int RY, int RW = SW3 + 2 * RX, int XOFF = 0>

@@ -1,4 +1,4 @@
-// cv_b200/csrc/common.cuh -- shared declarations for libcvb200.so (sm_100a only).
+// cv_b200/csrc/common.cuh -- shared declarations for libcvb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -19,7 +19,7 @@ struct cvb_ctx {
     uint64_t launches = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     cudaEvent_t ev_wait = nullptr;   // blocking-sync event of cvb_wait
-    int num_sms = 148;
+    int num_sms = 132;
     AkazeWorkspace *akaze = nullptr;
     MatchWorkspace *match = nullptr;
     GeomWorkspace *geom = nullptr;

@@ -83,7 +83,7 @@ int cvb_ctx_profile_report(cvb_ctx *ctx, char *buf, size_t cap) {
     return 0;
 }
 
-const char *cvb_version(void) { return "cvb200 0.1.0 (sm_100a)"; }
+const char *cvb_version(void) { return "cvb200 0.1.0 (sm_90a)"; }
 
 int cvb_ctx_create_on_stream(int device, void *cuda_stream, cvb_ctx **out) {
     if (!out) return CVB_EINVAL;
@@ -94,7 +94,7 @@ int cvb_ctx_create_on_stream(int device, void *cuda_stream, cvb_ctx **out) {
     if (cudaSetDevice(device) != cudaSuccess) return CVB_ENODEV;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return CVB_ENODEV;
-    if (prop.major < 10) return CVB_ENODEV;   // kernels are built for sm_100a only
+    if (prop.major != 9 || prop.minor != 0) return CVB_ENODEV;   // kernels are built for sm_90a only
     cvb_ctx *ctx = new cvb_ctx();
     ctx->device = device;
     ctx->num_sms = prop.multiProcessorCount;

@@ -1,9 +1,9 @@
-// cv_b200/csrc/geom.cu -- batched geometric verification on sm_100a (f64).
+// cv_b200/csrc/geom.cu -- batched geometric verification on sm_90a (f64).
 //
 // Every model hypothesis (eight-point / P3P minimal solve) and every (hypothesis, datum) residual runs on
 // the GPU, one thread per hypothesis resp. per (hypothesis, datum) pair; ARRSAC's inherently sequential
 // bookkeeping (likelihood-ratio test over hypotheses, sort / truncate, RNG draws) stays on the host and
-// consumes bit-packed inlier masks.  Reference lines are cited per function (paths relative to /root/reference).
+// consumes bit-packed inlier masks.  Reference lines are cited per function (paths relative to the reference checkout).
 // The linear algebra that lives in nalgebra upstream (symmetric eigen, SVD, from_matrix_eps) is implemented
 // here as cyclic Jacobi / closed forms; f64 results are held to 1e-6 relative (BASELINE north_star) in the parity tests.
 #include <math.h>
@@ -486,7 +486,7 @@ __device__ int p3p(const double *bearings, const double *world, const uint32_t *
 // reproduces the reference, row0 = 6 is the mathematically correct solver (see DESIGN.md).
 constexpr int FPN = 10;
 // __noinline__: with every helper inlined into one five-point frame, nvcc 12.9 -O3 produced a wrong complete-pivoting
-// elimination on sm_100a (the same text is right stand-alone and on the host); separate frames are bit-identical to the CPU.
+// elimination on sm_90a (the same text is right stand-alone and on the host); separate frames are bit-identical to the CPU.
 __device__ __noinline__ bool lu_full_pivot_solve(const double *Ain, const double *Bin, double *X) {
     double A[FPN][FPN], B[FPN][FPN];
     int colperm[FPN];
@@ -1599,10 +1599,10 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
-        // the initial scoring fills the machine (4 CTAs per SM).  A block scores ~200 k predicates; measured on B200 per pair (76 launches,
-    // most of them idle because the loop is over): 1.23 ms on 48 CTAs, 0.88 ms on 148, 0.79 ms on 296 for ONE context -- but 16
-    // pipelined contexts reach 1 678 / 1 660 / 1 629 frames/s: the small grid costs the least SM time (more units per warp, the
-    // exact-fallback stragglers amortised), and the step is bound by SM time, not by a pair's latency.  CVB_ARS_SGRID overrides.
+        // the initial scoring fills the machine (4 CTAs per SM).  A block scores ~200 k predicates on 48 CTAs: a larger grid
+    // lowers ONE context's latency, but with 16 pipelined contexts the small grid costs the least SM time (more units per warp, the
+    // exact-fallback stragglers amortised), and the step is bound by SM time, not by a pair's latency (not re-tuned on H100).
+    // CVB_ARS_SGRID overrides.
     const uint32_t sgrid_full = (uint32_t)ctx->num_sms * 4;
         uint32_t sgrid_block = 48;
         if (const char *e = getenv("CVB_ARS_SGRID")) sgrid_block = (uint32_t)std::max(1, atoi(e));

@@ -1,7 +1,7 @@
-// cv_b200/csrc/match.cu -- brute-force Hamming k-NN over 64-byte descriptors (sm_100a).
+// cv_b200/csrc/match.cu -- brute-force Hamming k-NN over 64-byte descriptors (sm_90a).
 //
 // Replaces `space::LinearKnn{metric: bitarray::Hamming, iter}.knn(query, k)` (external crates space 0.17 /
-// bitarray 0.9; call sites /root/reference/akaze/tests/estimate_pose.rs:78-97, tutorial-code/
+// bitarray 0.9; call sites akaze/tests/estimate_pose.rs:78-97, tutorial-code/
 // chapter4-feature-matching/src/main.rs:91-106, cv-sfm/src/lib.rs:3097-3114) for ALL queries at once.
 // Semantics kept bit-exact: distance = popcount(a ^ b) over 512 bits; the k smallest in ascending
 // distance; among equal distances the lower database index comes first.
@@ -25,7 +25,7 @@ constexpr int QT = 128;          // queries per CTA (1 per thread)
 constexpr int DTILE = 128;       // database descriptors per shared-memory tile (8 KB)
 constexpr int MAXKNN = 8;
 #ifndef CVB_KNN_DEFAULT_MODE
-#define CVB_KNN_DEFAULT_MODE 2     // 1: mma.sync int8, 2: tcgen05 (CVB_KNN_UMMA=1 / =0 override at run time)
+#define CVB_KNN_DEFAULT_MODE 2     // 1: mma.sync int8, 2: wgmma (CVB_KNN_WGMMA=1 / =0 override at run time)
 #endif
 constexpr unsigned IDX_BITS = 22;
 constexpr unsigned IDX_MASK = (1u << IDX_BITS) - 1u;
@@ -265,7 +265,7 @@ __global__ void __launch_bounds__(IM_WARPS * 32) k_hamming_imma(const uint8_t *_
     }
 }
 
-#include "match_umma.cuh"
+#include "match_wgmma.cuh"
 
 // merge the per-split lists (split order == index order) into global (idx, dist)
 template <int K>
@@ -386,7 +386,7 @@ struct MatchWorkspace {
     uint8_t *uq = nullptr, *udb = nullptr;         // unpacked (int8 0/1) descriptors for the tensor-core path
     uint16_t *pq = nullptr, *pdb = nullptr;
     size_t uq_bytes = 0, udb_bytes = 0, pq_elems = 0, pdb_elems = 0;
-    int use_imma = -1;                              // 2 tcgen05 (default), 1 mma.sync (CVB_KNN_IMMA=1), 0 popcount (CVB_KNN_POPC=1)
+    int use_imma = -1;                              // 2 wgmma (default), 1 mma.sync (CVB_KNN_IMMA=1), 0 popcount (CVB_KNN_POPC=1)
 };
 
 void match_workspace_free(MatchWorkspace *ws) {
@@ -446,14 +446,14 @@ int launch_knn_imma(cvb_ctx *ctx, MatchWorkspace *ws, const uint8_t *q, const ui
 }
 
 template <int K>
-int launch_knn_umma(cvb_ctx *ctx, MatchWorkspace *ws, const uint8_t *q, const uint32_t *n_dev, uint32_t n, const uint8_t *db,
-                    const uint32_t *m_dev, uint32_t m, uint32_t splits, uint32_t chunk, uint32_t *idx, uint32_t *dist) {
+int launch_knn_wgmma(cvb_ctx *ctx, MatchWorkspace *ws, const uint8_t *q, const uint32_t *n_dev, uint32_t n, const uint8_t *db,
+                     const uint32_t *m_dev, uint32_t m, uint32_t splits, uint32_t chunk, uint32_t *idx, uint32_t *dist) {
     {
         static bool attr_set = false;   // per template instance, once per process
-        if (!attr_set) { cudaFuncSetAttribute(umma::k_hamming_umma<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)umma::SMEM); attr_set = true; }
-        dim3 grid(cdiv(n, umma::QT), splits);
+        if (!attr_set) { cudaFuncSetAttribute(wg::k_hamming_wgmma<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wg::SMEM); attr_set = true; }
+        dim3 grid(cdiv(n, wg::QT), splits);
         CVB_PROF(ctx, "k_hamming_knn", 64.0 * (double)n * (double)m);
-        umma::k_hamming_umma<K><<<grid, umma::THREADS, umma::SMEM, ctx->stream>>>(q, n_dev, n, db, m_dev, m, chunk, ws->partial);
+        wg::k_hamming_wgmma<K><<<grid, wg::THREADS, wg::SMEM, ctx->stream>>>(q, n_dev, n, db, m_dev, m, chunk, ws->partial);
         CVB_LAUNCH_CHECK(ctx);
     }
     k_knn_merge<K><<<cdiv(n, 128), 128, 0, ctx->stream>>>(ws->partial, n_dev, n, splits, chunk, idx, dist);
@@ -468,29 +468,29 @@ int knn_dev(cvb_ctx *ctx, const uint8_t *q, const uint32_t *n_dev, uint32_t n, c
     if (((uintptr_t)q & 15) || ((uintptr_t)db & 15)) return cvb_set_error(ctx, CVB_EINVAL, "descriptor arrays must be 16-byte aligned");
     if (!ctx->match) ctx->match = new MatchWorkspace();
     MatchWorkspace *ws = ctx->match;
-    if (ws->use_imma < 0) {     // 2: tcgen05 (default), 1: legacy mma.sync int8 (CVB_KNN_IMMA=1), 0: popcount (CVB_KNN_POPC=1)
-        const char *env = getenv("CVB_KNN_POPC"), *env2 = getenv("CVB_KNN_IMMA"), *env3 = getenv("CVB_KNN_UMMA");
+    if (ws->use_imma < 0) {     // 2: wgmma (default), 1: legacy mma.sync int8 (CVB_KNN_IMMA=1), 0: popcount (CVB_KNN_POPC=1)
+        const char *env = getenv("CVB_KNN_POPC"), *env2 = getenv("CVB_KNN_IMMA"), *env3 = getenv("CVB_KNN_WGMMA");
         ws->use_imma = (env && env[0] == '1') ? 0 : ((env2 && env2[0] == '1') ? 1 : ((env3 && env3[0] == '0') ? 1 : (env3 && env3[0] == '1') ? 2 : CVB_KNN_DEFAULT_MODE));
     }
     if (ws->use_imma == 2 && m > 0) {
-        // tcgen05 path: 128-query CTAs (one per SM: 217 KB of shared memory); the database is split so that the grid is one wave
-        const uint32_t qblocks = cdiv(n, umma::QT);
+        // wgmma path: 128-query CTAs (one per SM: 145 KB of shared memory); the database is split so that the grid is one wave
+        const uint32_t qblocks = cdiv(n, wg::QT);
         uint32_t splits = std::max<uint32_t>(1, (uint32_t)ctx->num_sms / qblocks);
-        splits = std::min<uint32_t>(splits, std::max<uint32_t>(1, cdiv(m, umma::DT)));
-        uint32_t chunk = cdiv(cdiv(m, splits), umma::DT) * umma::DT;
-        while (chunk > IDX_MASK) { splits *= 2; chunk = cdiv(cdiv(m, splits), umma::DT) * umma::DT; }
+        splits = std::min<uint32_t>(splits, std::max<uint32_t>(1, cdiv(m, wg::DT)));
+        uint32_t chunk = cdiv(cdiv(m, splits), wg::DT) * wg::DT;
+        while (chunk > IDX_MASK) { splits *= 2; chunk = cdiv(cdiv(m, splits), wg::DT) * wg::DT; }
         splits = cdiv(m, chunk);
         int rc;
         if ((rc = grow(ctx, &ws->partial, &ws->partial_elems, (size_t)n * splits * k))) return rc;
         switch (k) {
-        case 1: return launch_knn_umma<1>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 2: return launch_knn_umma<2>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 3: return launch_knn_umma<3>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 4: return launch_knn_umma<4>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 5: return launch_knn_umma<5>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 6: return launch_knn_umma<6>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        case 7: return launch_knn_umma<7>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
-        default: return launch_knn_umma<8>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 1: return launch_knn_wgmma<1>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 2: return launch_knn_wgmma<2>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 3: return launch_knn_wgmma<3>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 4: return launch_knn_wgmma<4>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 5: return launch_knn_wgmma<5>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 6: return launch_knn_wgmma<6>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        case 7: return launch_knn_wgmma<7>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
+        default: return launch_knn_wgmma<8>(ctx, ws, q, n_dev, n, db, m_dev, m, splits, chunk, idx, dist);
         }
     }
     if (ws->use_imma == 1 && m > 0) {

@@ -1,4 +1,4 @@
-/* include/cvb200.h -- C ABI of libcvb200.so: the B200-native drop-in for rust-cv's
+/* include/cvb200.h -- C ABI of libcvb200.so: the H100-native drop-in for rust-cv's
  * AKAZE -> brute-force Hamming match -> RANSAC hot path.
  *
  * The reference (rust-cv/cv @ 82a25ee3) has no FFI; its boundary is the Rust-level API listed

@@ -3,7 +3,7 @@
  * This is the parity oracle (and the "port" CPU baseline) for the AKAZE extractor.  It is
  * NOT product code: only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
  * --impl reference legs may load it.  Every function cites the reference lines it follows
- * (paths relative to /root/reference/akaze/src).
+ * (paths relative to the reference's akaze/src).
  *
  * Pinning: tests/test_oracle_akaze.py checks this file against the reference's own goldens
  * (akaze/tests/estimate_pose.rs:41-42,59 -> 399 / 343 descriptors, 11 Lowe matches;

@@ -1,7 +1,7 @@
 /* oracle/ref_geom.c -- TEST INFRASTRUCTURE: CPU restatement of the geometric-verification half of the
  * hot path (SURVEY.md section 8a rows R1-R8, T1, C1).  Not product code.
  *
- * Follows (paths relative to /root/reference):
+ * Follows (paths relative to the reference checkout):
  *   eight-point/src/lib.rs:11-84            encode_epipolar_equation (incl. the b/a.z quirk), from_matches, estimate
  *   cv-pinhole/src/essential.rs:114-231     possible_rotations_unscaled_translation / possible_unscaled_poses
  *   cv-pinhole/src/essential.rs:266-275     EssentialMatrix::residual
@@ -10,7 +10,7 @@
  *   cv-core/src/point.rs:20-25              Projective::from_homogeneous
  *   lambda-twist/src/lib.rs:110-317,361-554 compute_poses_nordberg and helpers
  *   cv-geom/src/triangulation.rs:82-130     LinearEigenTriangulator
- * and, from crates that are NOT in /root/reference (restated from their published algorithms):
+ * and, from crates that are NOT in the reference checkout (restated from their published algorithms):
  *   nalgebra 0.30.1   try_symmetric_eigen / SVD  -> here: cyclic Jacobi (same mathematical result up to the
  *                     sign/order of eigenvectors, which nalgebra does not specify either); Rotation3::from_matrix_eps
  *   arrsac 0.10.0     adaptive real-time RANSAC   -> ref_arrsac_* below: restated from the crate's documented

@@ -2,8 +2,8 @@
  *
  * Follows `space::LinearKnn{metric: Hamming, iter}.knn(query, k)` (external crate space 0.17.0)
  * with `bitarray::Hamming` over `BitArray<64>` (external crate bitarray 0.9.0), as called at
- * /root/reference/akaze/tests/estimate_pose.rs:78-97 and tutorial-code/chapter4-feature-matching/
- * src/main.rs:91-106.  Neither crate's source is in /root/reference; the published algorithm is:
+ * akaze/tests/estimate_pose.rs:78-97 and tutorial-code/chapter4-feature-matching/
+ * src/main.rs:91-106.  Neither crate's source is in the reference checkout; the published algorithm is:
  * distance = sum popcount(a[i]^b[i]) over 64 bytes (u32); knn keeps the k smallest in ascending
  * distance, and among equal distances the EARLIER database index stays first (insert position =
  * partition_point(|n| n.distance <= d)).  Pinned by the reference's own golden: 11 Lowe-ratio

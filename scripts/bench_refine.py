@@ -19,10 +19,10 @@ out = {}
 # ---- single-view L2 refinement: cv-sfm's sizes (<= 2048 matches, rate 1e-3), fixed iteration count
 N, IT = 2048, 2000
 probs = []
-for b in range(148):
+for b in range(132):
     R, t, bearings, world, _ = pnp_scene(rng, N, noise=2e-4)
     probs.append((perturb_pose(rng, (R, t), 2e-3, 5e-3), bearings, world))
-for B in (1, 16, 148):
+for B in (1, 16, 132):
     poses = [p[0] for p in probs[:B]]
     bearings = np.concatenate([p[1] for p in probs[:B]]); world = np.concatenate([p[2] for p in probs[:B]])
     off = np.arange(B + 1) * N
@@ -40,10 +40,10 @@ out["single_view_cpu_B1"] = {"ms": dt * 1e3, "updates": int(uw), "us_per_iterati
 # ---- three-view L2 refinement: 1024 landmarks (cv-sfm three_view_optimization_landmarks)
 N3, IT3 = 1024, 1000
 p3 = []
-for b in range(148):
+for b in range(132):
     truth, obs = three_view_scene(rng, N3, noise=1e-4)
     p3.append(([perturb_pose(rng, p, 3e-3, 5e-3) for p in truth], obs))
-for B in (1, 148):
+for B in (1, 132):
     starts = [p[0] for p in p3[:B]]; obs = np.concatenate([p[1] for p in p3[:B]]); off = np.arange(B + 1) * N3
     cv_b200.three_view_optimize_l2_batch(starts, 1e-3, 10, obs, off)
     t0 = time.perf_counter()

@@ -1,5 +1,5 @@
 """Per-kernel CUDA-event times of one frame pair (extract x2 -> symmetric match -> bearings -> ARRSAC), single context, no overlap.
-python scripts/prof_kernels.py [pairs]   (env CVB_TMA / CVB_KNN_UMMA select the variants)"""
+python scripts/prof_kernels.py [pairs]   (env CVB_TMA / CVB_KNN_WGMMA select the variants)"""
 import ctypes as C, json, os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -44,7 +44,7 @@ for i in range(pairs):
 rep = ctx.profile_report()
 ctx.profile(False)
 tot = sum(v["ms"] for v in rep.values())
-print(json.dumps({"tma": os.environ.get("CVB_TMA"), "umma": os.environ.get("CVB_KNN_UMMA"), "single_context_ms_per_pair": ms_graph,
+print(json.dumps({"tma": os.environ.get("CVB_TMA"), "wgmma": os.environ.get("CVB_KNN_WGMMA"), "single_context_ms_per_pair": ms_graph,
                   "sum_kernel_ms_per_pair": tot / pairs, "counts": cnt.cpu().tolist(), "stats": [int(x) for x in stats]}))
 for k, v in sorted(rep.items(), key=lambda kv: -kv[1]["ms"]):
     print(f"{k:28s} {v['ms'] / pairs:9.4f} ms/pair  {v['launches'] / pairs:7.1f} launches")

@@ -1,8 +1,8 @@
-"""Generates the golden fixtures under tests/golden/ (run in the build container, where
-/root/reference exists; the GPU box never reads /root/reference).
+"""Generates the golden fixtures under tests/golden/ from a checkout of rust-cv/cv @ 82a25ee3:
+python tests/golden/make_golden.py <rust-cv checkout>.  The tests read only the committed fixtures.
 
  - kitti_0000000000.npz / kitti_0000000014.npz : the two reference fixture frames
-   (/root/reference/res/*.png, 1392x512 8-bit gray) as uint8 arrays -- inputs of the reference's
+   (res/*.png of the checkout, 1392x512 8-bit gray) as uint8 arrays -- inputs of the reference's
    own golden test akaze/tests/estimate_pose.rs:24-76.
  - akaze_goldens.json : the counts that test asserts (399 / 343 descriptors, 11 Lowe-0.5 matches,
    estimate_pose.rs:41-42,59) plus secondary counts produced by the oracle at Akaze::default().
@@ -20,10 +20,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "..", ".."))
 from oracle import pyoracle as O  # noqa: E402
 
-REF = "/root/reference/res"
 
 
 def main():
+    REF = os.path.join(sys.argv[1], "res")
     frames = {}
     for name in ("0000000000", "0000000014"):
         im = cv2.imread(os.path.join(REF, name + ".png"), cv2.IMREAD_UNCHANGED)

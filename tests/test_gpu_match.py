@@ -98,12 +98,12 @@ def test_landmark_matches_against_loop_restatement():
     assert cv_b200.landmark_matches(new, views, 24) == O.landmark_matches_ref(new, views, 24)
 
 
-@pytest.mark.parametrize("mode", ["umma", "imma", "popc"])
+@pytest.mark.parametrize("mode", ["wgmma", "imma", "popc"])
 def test_three_matcher_kernels_agree_with_oracle(mode, monkeypatch):
-    """tcgen05 (UTCIMMA + TMEM, default), legacy mma.sync int8 and popcount kernels: identical k-NN tables, ragged sizes included"""
-    for k_ in ("CVB_KNN_UMMA", "CVB_KNN_IMMA", "CVB_KNN_POPC"):
+    """wgmma (default), legacy mma.sync int8 and popcount kernels: identical k-NN tables, ragged sizes included"""
+    for k_ in ("CVB_KNN_WGMMA", "CVB_KNN_IMMA", "CVB_KNN_POPC"):
         monkeypatch.delenv(k_, raising=False)
-    monkeypatch.setenv({"umma": "CVB_KNN_UMMA", "imma": "CVB_KNN_IMMA", "popc": "CVB_KNN_POPC"}[mode], "1")
+    monkeypatch.setenv({"wgmma": "CVB_KNN_WGMMA", "imma": "CVB_KNN_IMMA", "popc": "CVB_KNN_POPC"}[mode], "1")
     ctx = cv_b200.Context(0)          # the kernel choice is latched per context at its first k-NN call
     for n, m, k in [(1, 1, 1), (129, 127, 2), (300, 1000, 3), (1000, 300, 2), (640, 2049, 8)]:
         q, db = random_descriptors(n, 100 + n), random_descriptors(m, 200 + m)
