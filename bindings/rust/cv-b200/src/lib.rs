@@ -174,3 +174,8 @@ impl TriangulatorObservations for CudaLinearEigen {
         self.triangulate_batch(&poses, &bearings, &[0, poses.len() as u32]).pop().flatten()
     }
 }
+
+
+// ---- INTEGRATION.md section 2c (include/cvb200_sfm.h) ----
+mod sfm;
+pub use sfm::*;

@@ -6,6 +6,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   KeyPoint dtype        <- akaze::KeyPoint                    (akaze/src/lib.rs:71-93)
   LinearKnn / hamming_knn <- space::LinearKnn + bitarray::Hamming (call sites akaze/tests/estimate_pose.rs:78-97)
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
+  CameraIntrinsics(K1Distortion) <- cv-pinhole/src/lib.rs:32-240
+  frame_features        <- cv-sfm VSlam::kps_descriptors        (cv-sfm/src/lib.rs:2195-2235)
 
 There is no CPU fallback: every call runs CUDA kernels from cv_b200/libcvb200.so and raises
 CvbError when the library or a Hopper (sm_90) GPU is missing.
@@ -13,7 +15,7 @@ CvbError when the library or a Hopper (sm_90) GPU is missing.
 from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F401
 from .akaze import Akaze, AkazeConfig  # noqa: F401
 from .knn import HammingHasher, LinearKnn, hamming_knn, lowe_ratio_matches, matching, symmetric_matching  # noqa: F401
-from .pinhole import CameraIntrinsics  # noqa: F401
+from .pinhole import CameraIntrinsics, CameraIntrinsicsK1Distortion  # noqa: F401
 from .geom import (Arrsac, EightPoint, LambdaTwist, LinearEigenTriangulator, NisterStewenius, Pcg64, Xoshiro256PlusPlus,  # noqa: F401
                    residuals_camera_to_camera, residuals_world_to_camera)
 from .optimize import (observation_losses, single_view_simple_optimize_l2, single_view_simple_optimize_l2_batch,  # noqa: F401
@@ -21,6 +23,7 @@ from .optimize import (observation_losses, single_view_simple_optimize_l2, singl
                        tri_landmarks_robust)
 from .sfm_match import landmark_matches  # noqa: F401
 from . import checkpoint  # noqa: F401  (bincode record images of the VSlamData checkpoint)
-from .pair import Intrinsics, TwoViewBuffers, two_view_frames  # noqa: F401
+from .pair import Intrinsics, IntrinsicsK1, TwoViewBuffers, two_view_frames  # noqa: F401
+from .features import frame_features  # noqa: F401
 
 __version__ = "0.1.0"

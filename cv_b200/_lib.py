@@ -54,6 +54,11 @@ ABI_SYMBOLS = [
     "cvb_single_view_optimize_l2", "cvb_three_view_optimize_l2", "cvb_observation_losses", "cvb_tri_landmarks_robust",
 ]
 
+# every symbol include/cvb200_sfm.h declares (the K1 camera and cv-sfm's frame ingestion; checked by tests/test_abi_sfm.py)
+SFM_ABI_SYMBOLS = [
+    "cvb_pair_bearings_k1_dev", "cvb_two_view_pair_k1_dev", "cvb_two_view_frames_k1", "cvb_frame_features_batch", "cvb_frame_features_batch_dev",
+]
+
 
 def lib_path():
     return os.path.join(_HERE, "libcvb200.so")

@@ -4,12 +4,13 @@
 #include <stdint.h>
 #include <string>
 #include <vector>
-#include "../../include/cvb200.h"
+#include "../../include/cvb200_sfm.h"   // includes cvb200.h
 
 struct AkazeWorkspace;
 struct MatchWorkspace;
 struct GeomWorkspace;
 struct PairWorkspace;
+struct FrameWorkspace;
 
 struct cvb_ctx {
     int device = 0;
@@ -24,6 +25,7 @@ struct cvb_ctx {
     MatchWorkspace *match = nullptr;
     GeomWorkspace *geom = nullptr;
     PairWorkspace *pair = nullptr;
+    FrameWorkspace *frame = nullptr;
     // page-locked host scratch for the small device->host results of the host API (a D2H copy into pageable memory is
     // staged synchronously inside the driver and stalls the other contexts' launches)
     void *pinned = nullptr;
@@ -58,6 +60,7 @@ void akaze_workspace_free(AkazeWorkspace *ws);
 void match_workspace_free(MatchWorkspace *ws);
 void geom_workspace_free(GeomWorkspace *ws);
 void pair_workspace_free(PairWorkspace *ws);
+void frame_workspace_free(FrameWorkspace *ws);
 
 #define CVB_CUDA(ctx, call)                                                                          \
     do {                                                                                             \

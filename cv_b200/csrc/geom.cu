@@ -14,6 +14,7 @@
 #include <vector>
 #include "common.cuh"
 #include "c2c_filter.cuh"
+#include "pinhole.cuh"
 
 namespace {
 
@@ -855,21 +856,15 @@ __global__ void __launch_bounds__(128) k_triangulate(const cvb_pose *__restrict_
 
 // cv-sfm keeps calibrated bearings per feature (CameraModel::calibrate, cv-pinhole/src/lib.rs:108-116, on
 // akaze::KeyPoint's ImagePoint, akaze/src/lib.rs:95-99); a FeatureMatch is the bearing pair of a match (cv-sfm/src/lib.rs:1400).
-// One thread per match: both bearings in f64 with the reference's operation order (no distortion: k1 = 0).
-__device__ __forceinline__ void calibrate_px(const cvb_intrinsics K, double px, double py, double *o) {
-    const double y = (py - K.cy) / K.fy;
-    const double x = (px - K.cx - K.skew * y) / K.fx;
-    const double n = sqrt(x * x + y * y + 1.0);
-    o[0] = x / n; o[1] = y / n; o[2] = 1.0 / n;
-}
+// One thread per match: both bearings in f64 with the reference's operation order (pinhole.cuh; k1 = 0 for CameraIntrinsics).
 __global__ void __launch_bounds__(256) k_pair_bearings(const cvb_keypoint *__restrict__ kpa, const cvb_keypoint *__restrict__ kpb,
                                                        const uint32_t *__restrict__ pairs, const uint32_t *__restrict__ npairs,
-                                                       uint32_t cap, cvb_intrinsics K, double *__restrict__ a, double *__restrict__ b) {
+                                                       uint32_t cap, cvb_intrinsics_k1 K, double *__restrict__ a, double *__restrict__ b) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= min(*npairs, cap)) return;
     const cvb_keypoint ka = kpa[pairs[2 * i]], kb = kpb[pairs[2 * i + 1]];
-    calibrate_px(K, (double)ka.x, (double)ka.y, a + 3 * (size_t)i);
-    calibrate_px(K, (double)kb.x, (double)kb.y, b + 3 * (size_t)i);
+    calibrate_k1(K, (double)ka.x, (double)ka.y, a + 3 * (size_t)i);
+    calibrate_k1(K, (double)kb.x, (double)kb.y, b + 3 * (size_t)i);
 }
 
 #include "arrsac_dev.cuh"
@@ -2044,6 +2039,12 @@ int cvb_arrsac_p3p(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, const double *bearin
 // ---- device-resident entry points (asynchronous on the context stream) -----------------------------------------------------
 int cvb_pair_bearings_dev(cvb_ctx *ctx, const cvb_keypoint *kp_a_dev, const cvb_keypoint *kp_b_dev, const uint32_t *pairs_dev,
                           const uint32_t *n_pairs_dev, uint32_t cap, const cvb_intrinsics *intrinsics, double *a_out_dev, double *b_out_dev) {
+    const cvb_intrinsics_k1 K = intrinsics ? intrinsics_k1(*intrinsics) : cvb_intrinsics_k1{};
+    return cvb_pair_bearings_k1_dev(ctx, kp_a_dev, kp_b_dev, pairs_dev, n_pairs_dev, cap, intrinsics ? &K : nullptr, a_out_dev, b_out_dev);
+}
+int cvb_pair_bearings_k1_dev(cvb_ctx *ctx, const cvb_keypoint *kp_a_dev, const cvb_keypoint *kp_b_dev, const uint32_t *pairs_dev,
+                             const uint32_t *n_pairs_dev, uint32_t cap, const cvb_intrinsics_k1 *intrinsics, double *a_out_dev,
+                             double *b_out_dev) {
     if (!ctx) return CVB_EINVAL;
     if (!kp_a_dev || !kp_b_dev || !pairs_dev || !n_pairs_dev || !intrinsics || !a_out_dev || !b_out_dev) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
     if (cap == 0) return 0;

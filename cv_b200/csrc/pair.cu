@@ -4,6 +4,7 @@
 #include <string.h>
 #include <algorithm>
 #include "common.cuh"
+#include "pinhole.cuh"
 
 struct PairWorkspace {
     float *img = nullptr; size_t img_floats = 0;
@@ -60,11 +61,31 @@ int ensure_pair(cvb_ctx *ctx, uint32_t cap, size_t img_floats) {
 
 extern "C" {
 
+// The entry points taking cvb_intrinsics are the K1 ones with k1 = 0 (bit-identical bearings, pinhole.cuh).
 int cvb_two_view_pair_dev(cvb_ctx *ctx, const cvb_keypoint *kp_a_dev, const uint8_t *desc_a_dev, const uint32_t *n_a_dev,
                           const cvb_keypoint *kp_b_dev, const uint8_t *desc_b_dev, const uint32_t *n_b_dev, uint32_t n_max,
                           uint32_t better_by, const cvb_intrinsics *intrinsics, const cvb_arrsac_cfg *cfg, const cvb_rng *rng,
                           uint32_t *pairs_out_dev, uint32_t cap, uint32_t *n_pairs_dev, cvb_pose *model_out_dev,
                           uint32_t *inliers_out_dev, uint32_t *n_inliers_dev, int32_t *found_dev) {
+    const cvb_intrinsics_k1 K = intrinsics ? intrinsics_k1(*intrinsics) : cvb_intrinsics_k1{};
+    return cvb_two_view_pair_k1_dev(ctx, kp_a_dev, desc_a_dev, n_a_dev, kp_b_dev, desc_b_dev, n_b_dev, n_max, better_by, intrinsics ? &K : nullptr,
+                                    cfg, rng, pairs_out_dev, cap, n_pairs_dev, model_out_dev, inliers_out_dev, n_inliers_dev, found_dev);
+}
+
+int cvb_two_view_frames(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *frames, uint32_t w, uint32_t h, uint32_t better_by,
+                        const cvb_intrinsics *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng, cvb_keypoint *kp_out, uint8_t *desc_out,
+                        uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs, cvb_pose *model_out, uint32_t *inliers_out,
+                        uint32_t *n_inliers, int32_t *found) {
+    const cvb_intrinsics_k1 K = intrinsics ? intrinsics_k1(*intrinsics) : cvb_intrinsics_k1{};
+    return cvb_two_view_frames_k1(ctx, akaze, frames, w, h, better_by, intrinsics ? &K : nullptr, cfg, rng, kp_out, desc_out, cap, n_out,
+                                  pairs_out, n_pairs, model_out, inliers_out, n_inliers, found);
+}
+
+int cvb_two_view_pair_k1_dev(cvb_ctx *ctx, const cvb_keypoint *kp_a_dev, const uint8_t *desc_a_dev, const uint32_t *n_a_dev,
+                             const cvb_keypoint *kp_b_dev, const uint8_t *desc_b_dev, const uint32_t *n_b_dev, uint32_t n_max,
+                             uint32_t better_by, const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, const cvb_rng *rng,
+                             uint32_t *pairs_out_dev, uint32_t cap, uint32_t *n_pairs_dev, cvb_pose *model_out_dev,
+                             uint32_t *inliers_out_dev, uint32_t *n_inliers_dev, int32_t *found_dev) {
     if (!ctx) return CVB_EINVAL;
     if (!kp_a_dev || !desc_a_dev || !n_a_dev || !kp_b_dev || !desc_b_dev || !n_b_dev || !intrinsics || !cfg || !rng || !pairs_out_dev ||
         !n_pairs_dev || !model_out_dev || !n_inliers_dev || !found_dev)
@@ -75,14 +96,14 @@ int cvb_two_view_pair_dev(cvb_ctx *ctx, const cvb_keypoint *kp_a_dev, const uint
     PairWorkspace *w = ctx->pair;
     if ((rc = cvb_match_symmetric_pairs_dev(ctx, desc_a_dev, n_a_dev, n_max, desc_b_dev, n_b_dev, n_max, better_by, pairs_out_dev, cap, n_pairs_dev)))
         return rc;
-    if ((rc = cvb_pair_bearings_dev(ctx, kp_a_dev, kp_b_dev, pairs_out_dev, n_pairs_dev, cap, intrinsics, w->a, w->b))) return rc;
+    if ((rc = cvb_pair_bearings_k1_dev(ctx, kp_a_dev, kp_b_dev, pairs_out_dev, n_pairs_dev, cap, intrinsics, w->a, w->b))) return rc;
     return cvb_arrsac_eight_point_dev(ctx, cfg, w->a, w->b, n_pairs_dev, cap, rng, model_out_dev, inliers_out_dev, cap, n_inliers_dev, found_dev);
 }
 
-int cvb_two_view_frames(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *frames, uint32_t w, uint32_t h, uint32_t better_by,
-                        const cvb_intrinsics *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng, cvb_keypoint *kp_out, uint8_t *desc_out,
-                        uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs, cvb_pose *model_out, uint32_t *inliers_out,
-                        uint32_t *n_inliers, int32_t *found) {
+int cvb_two_view_frames_k1(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *frames, uint32_t w, uint32_t h, uint32_t better_by,
+                           const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng, cvb_keypoint *kp_out,
+                           uint8_t *desc_out, uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs, cvb_pose *model_out,
+                           uint32_t *inliers_out, uint32_t *n_inliers, int32_t *found) {
     if (!ctx) return CVB_EINVAL;
     if (!akaze || !frames || !intrinsics || !cfg || !rng || !kp_out || !desc_out || !n_out || !pairs_out || !n_pairs || !model_out ||
         !inliers_out || !n_inliers || !found)
@@ -101,8 +122,8 @@ int cvb_two_view_frames(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *f
     uint32_t *pairs_dev = (uint32_t *)(pw->res + L.pairs), *inl_dev = (uint32_t *)(pw->res + L.inliers);
     CVB_CUDA(ctx, cudaMemcpyAsync(pw->img, frames, sizeof(float) * 2 * px, cudaMemcpyHostToDevice, st));
     if ((rc = cvb_akaze_extract_batch_dev(ctx, akaze, pw->img, 2, w, h, pw->kp, pw->desc, pw->cap, pw->n))) return rc;
-    if ((rc = cvb_two_view_pair_dev(ctx, pw->kp, pw->desc, pw->n, pw->kp + pw->cap, pw->desc + (size_t)pw->cap * 64, pw->n + 1, pw->cap,
-                                    better_by, intrinsics, cfg, rng, pairs_dev, cap, n_pairs_dev, model_dev, inl_dev, n_inl_dev, found_dev)))
+    if ((rc = cvb_two_view_pair_k1_dev(ctx, pw->kp, pw->desc, pw->n, pw->kp + pw->cap, pw->desc + (size_t)pw->cap * 64, pw->n + 1, pw->cap,
+                                       better_by, intrinsics, cfg, rng, pairs_dev, cap, n_pairs_dev, model_dev, inl_dev, n_inl_dev, found_dev)))
         return rc;
     // results by capacity (the counts are only known on the device): one synchronisation at the very end
     unsigned char *hs = (unsigned char *)cvb_pinned(ctx, L.model + sizeof(cvb_pose) + 16);

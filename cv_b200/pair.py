@@ -7,6 +7,7 @@ import numpy as np
 
 from ._lib import KP_DTYPE, default_context
 from .geom import Arrsac, Pose, _lib as _geom_lib
+from .pinhole import CameraIntrinsicsK1Distortion
 
 
 class Intrinsics(C.Structure):
@@ -16,6 +17,18 @@ class Intrinsics(C.Structure):
     @classmethod
     def from_camera(cls, cam):
         return cls(cam.focals[0], cam.focals[1], cam.principal_point[0], cam.principal_point[1], cam.skew)
+
+
+class IntrinsicsK1(C.Structure):
+    """cvb_intrinsics_k1 == cv_pinhole::CameraIntrinsicsK1Distortion (simple intrinsics + k1)"""
+    _fields_ = Intrinsics._fields_ + [("k1", C.c_double)]
+
+    @classmethod
+    def from_camera(cls, cam):
+        """a CameraIntrinsicsK1Distortion, or a CameraIntrinsics (k1 = 0: the same bearings bit for bit)"""
+        k1 = getattr(cam, "k1", None)
+        s = cam.simple_intrinsics if k1 is not None else cam
+        return cls(s.focals[0], s.focals[1], s.principal_point[0], s.principal_point[1], s.skew, 0.0 if k1 is None else k1)
 
 
 def bind(L):
@@ -29,6 +42,11 @@ def bind(L):
     L.cvb_arrsac_commit_rng.argtypes = [vp, vp, vp]
     L.cvb_two_view_pair_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp, u32, u32, C.POINTER(Intrinsics), vp, vp, vp, u32, vp, vp, vp, vp, vp]
     L.cvb_two_view_frames.argtypes = [vp, vp, vp, u32, u32, u32, C.POINTER(Intrinsics), vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
+    L.cvb_pair_bearings_k1_dev.argtypes = [vp, vp, vp, vp, vp, u32, C.POINTER(IntrinsicsK1), vp, vp]
+    L.cvb_two_view_pair_k1_dev.argtypes = [vp, vp, vp, vp, vp, vp, vp, u32, u32, C.POINTER(IntrinsicsK1), vp, vp, vp, u32, vp, vp, vp, vp, vp]
+    L.cvb_two_view_frames_k1.argtypes = [vp, vp, vp, u32, u32, u32, C.POINTER(IntrinsicsK1), vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
+    L.cvb_frame_features_batch.argtypes = [vp, vp, vp, vp, u32, u32, u32, C.POINTER(IntrinsicsK1), vp, vp, vp, vp, u32, vp]
+    L.cvb_frame_features_batch_dev.argtypes = [vp, vp, vp, u32, u32, vp, u32, u32, C.POINTER(IntrinsicsK1), vp, vp]
     L._pair_bound = True
 
 
@@ -48,7 +66,8 @@ class TwoViewBuffers:
 
 
 def two_view_frames(akaze, frames, camera, arrsac, better_by=24, cap=8192, buffers=None):
-    """frames: [2, H, W] float32.  akaze: cv_b200.Akaze; camera: cv_b200.CameraIntrinsics; arrsac: cv_b200.Arrsac (its generator
+    """frames: [2, H, W] float32.  akaze: cv_b200.Akaze; camera: cv_b200.CameraIntrinsics (cvb_two_view_frames) or
+    cv_b200.CameraIntrinsicsK1Distortion (cvb_two_view_frames_k1); arrsac: cv_b200.Arrsac (its generator
     advances as the reference's would).  Returns dict(keypoints, descriptors, matches [[a, b], ...], pose (R, t) or None,
     inliers (indices into matches))."""
     frames = np.ascontiguousarray(frames, np.float32)
@@ -60,11 +79,14 @@ def two_view_frames(akaze, frames, camera, arrsac, better_by=24, cap=8192, buffe
     bind(L)
     b = buffers or TwoViewBuffers(cap)
     cfg = akaze.config.to_c()
-    K = Intrinsics.from_camera(camera)
-    ctx.check(L.cvb_two_view_frames(ctx.handle, C.addressof(cfg), frames.ctypes.data, frames.shape[2], frames.shape[1], better_by, C.byref(K),
-                                    C.addressof(arrsac.cfg), C.addressof(arrsac.rng.state), b.kp.ctypes.data, b.desc.ctypes.data, b.cap,
-                                    b.n.ctypes.data, b.pairs.ctypes.data, C.addressof(b.n_pairs), C.addressof(b.model), b.inliers.ctypes.data,
-                                    C.addressof(b.n_inliers), C.addressof(b.found)))
+    if isinstance(camera, CameraIntrinsicsK1Distortion):
+        K, entry = IntrinsicsK1.from_camera(camera), L.cvb_two_view_frames_k1
+    else:
+        K, entry = Intrinsics.from_camera(camera), L.cvb_two_view_frames
+    ctx.check(entry(ctx.handle, C.addressof(cfg), frames.ctypes.data, frames.shape[2], frames.shape[1], better_by, C.byref(K),
+                    C.addressof(arrsac.cfg), C.addressof(arrsac.rng.state), b.kp.ctypes.data, b.desc.ctypes.data, b.cap,
+                    b.n.ctypes.data, b.pairs.ctypes.data, C.addressof(b.n_pairs), C.addressof(b.model), b.inliers.ctypes.data,
+                    C.addressof(b.n_inliers), C.addressof(b.found)))
     kps = [b.kp[f, :b.n[f]].copy() for f in range(2)]
     descs = [b.desc[f, :b.n[f]].copy() for f in range(2)]
     pose = (np.array(b.model.r).reshape(3, 3), np.array(b.model.t)) if b.found.value else None

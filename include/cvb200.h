@@ -231,6 +231,7 @@ int cvb_arrsac_p3p(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, const double *bearin
  * *rng at call time (the generator is sequential; modulo and rejection run on the device because they need the datum count); the
  * caller's generator is advanced by the number of draws actually consumed with cvb_arrsac_commit_rng after the stream has drained. */
 typedef struct { double fx, fy, cx, cy, skew; } cvb_intrinsics;   /* cv_pinhole::CameraIntrinsics (cv-pinhole/src/lib.rs:32-41), k1 = 0 */
+/* (the camera with radial distortion, CameraIntrinsicsK1Distortion, and cv-sfm's frame ingestion: include/cvb200_sfm.h) */
 
 /* counts read from device memory (the n_out_dev of cvb_akaze_extract_batch_dev); pairs_out_dev: up to cap (a, b) index pairs in
  * ascending a; *n_pairs_dev <= cap */
