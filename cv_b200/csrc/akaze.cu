@@ -105,6 +105,7 @@ struct AkazeWorkspace {
     float *Lt = nullptr, *Lsm = nullptr, *Lx = nullptr, *Ly = nullptr, *Lflow = nullptr, *Ldet = nullptr;
     float *tmpA = nullptr, *tmpB = nullptr, *tmpC = nullptr;
     bool fuse_blur_scharr = true;   // one launch per evolution for Lsmooth + Lflow (CVB_NO_FUSE_BLUR=1: the two separate kernels)
+    bool fuse_det = true;           // one launch per octave for Lx, Ly, Ldet + extrema mask (CVB_NO_FUSE_DET=1: the three separate kernels)
     double *g2 = nullptr;
     unsigned long long *gmax = nullptr;
     unsigned *hist = nullptr, *npoints = nullptr;
@@ -430,6 +431,8 @@ int build_workspace(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, 
         ws->use_aux = !(env && env[0] == '1');
         env = getenv("CVB_NO_FUSE_BLUR");
         ws->fuse_blur_scharr = !(env && env[0] == '1');
+        env = getenv("CVB_NO_FUSE_DET");
+        ws->fuse_det = !(env && env[0] == '1');
         cudaStreamCreateWithFlags(&ws->aux, cudaStreamNonBlocking);
         for (auto &e : ws->ev_fork) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
         cudaEventCreateWithFlags(&ws->ev_join, cudaEventDisableTiming);
@@ -567,6 +570,9 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
     int smax = 1;
     for (const EvoHost &e : ws->evo) smax = std::max(smax, (int)e.sigma);
     const bool aux_ok = ws->use_aux && !ctx->prof;
+    const bool fused_det = ws->deriv_v3 && ws->fuse_det;   // the detector response writes the extrema mask itself
+    const int R = ws->table.total_rows;
+    const float thr = (float)ws->cfg.detector_threshold;
     bool forked = false;
     int fork_id = 0;
     // detector response (derivatives + Ldet) of evolutions [e0, e1): they only depend on Lsmooth of those evolutions
@@ -584,7 +590,14 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
         }
         double px = 0;
         for (int e = e0; e < e1; e++) px += (double)ws->evo[e].w * ws->evo[e].h;
-        if (ws->deriv_v3) {
+        if (fused_det) {
+            dim3 g((unsigned)(t1 - t0), 1, B);
+            CVB_PROF(ctx, "k_detector_response", 16.0 * px * B);
+            k_detector_response<<<g, NT, sizeof(float) * det_smem_floats(smax), ds>>>(ws->Lsm, ws->Lt, ws->Lx, ws->Ly, ws->Ldet, PF, ws->table,
+                                                                                      ws->tile_evo, t0, ws->mask_layout, thr, ws->extrema_mask,
+                                                                                      ws->rowcount);
+            CVB_LAUNCH_CHECK(ctx);
+        } else if (ws->deriv_v3) {
             const size_t region = (((size_t)pitch3(smax) * (SH3 + 2 * smax)) + 31) & ~(size_t)31;
             dim3 g((unsigned)(t1 - t0), 1, B);
             { CVB_PROF(ctx, "k_deriv1", 12.0 * px * B);
@@ -619,6 +632,8 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
     CVB_CUDA(ctx, cudaMemsetAsync(ws->gmax, 0, sizeof(unsigned long long) * B, st));
     CVB_CUDA(ctx, cudaMemsetAsync(ws->hist, 0, sizeof(unsigned) * B * nbins, st));
     CVB_CUDA(ctx, cudaMemsetAsync(ws->npoints, 0, sizeof(unsigned) * B, st));
+    // per-row extrema counts: ordered before the first fork, the fused detector response adds to them on the auxiliary stream
+    CVB_CUDA(ctx, cudaMemsetAsync(ws->rowcount, 0, sizeof(unsigned) * (size_t)B * R, st));
     rc = launch_separable(ctx, images, P0, ws->tmpA, P0, W, H, B, ws->g1, ws->g1);
     if (rc) return rc;
     { CVB_PROF(ctx, "k_contrast_grad", 4.0 * W * H * B);
@@ -699,11 +714,8 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
         CVB_CUDA(ctx, cudaStreamWaitEvent(st, ws->ev_join, 0));
     }
     // ---- detect_keypoints (scale_space_extrema.rs)
-    const int R = ws->table.total_rows;
-    const float thr = (float)ws->cfg.detector_threshold;
     {
-        CVB_CUDA(ctx, cudaMemsetAsync(ws->rowcount, 0, sizeof(unsigned) * (size_t)B * R, st));
-        { CVB_PROF(ctx, "k_extrema_mask", 4.0 * ws->plane_floats * B);
+        if (!fused_det) { CVB_PROF(ctx, "k_extrema_mask", 4.0 * ws->plane_floats * B);
         k_extrema_mask<<<dim3((unsigned)ws->table.total_tiles, 1, B), NT, 0, st>>>(ws->Ldet, PF, ws->table, ws->tile_evo, ws->mask_layout, thr,
                                                                                     ws->extrema_mask, ws->rowcount);
         CVB_LAUNCH_CHECK(ctx); }

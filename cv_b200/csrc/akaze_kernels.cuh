@@ -854,6 +854,166 @@ __global__ void __launch_bounds__(NT) k_extrema_mask(const float *__restrict__ L
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Detector response of one tile in ONE pass (detector_response.rs:40-68 + scale_space_extrema.rs:49-59): the work of
+// k_deriv1_v3 + k_deriv2_v3 + k_extrema_mask without the Lx / Ly / Ldet re-reads.  Lsmooth is staged with a halo of 2S+1;
+// Lx, Ly are computed over the tile plus a ring of S+1 (the tile part written to the planes), Ldet over the tile plus a
+// one-pixel ring (the tile part written to the plane), and the 3x3 test runs on that Ldet tile in shared memory.
+// Ring positions of Lx / Ly outside the image take the value at the clamped position, which is what k_deriv2_v3's
+// replicate-border staging of the Lx / Ly planes reads (as k_blur_scharr_pm does for Lsmooth).  Ldet ring positions outside
+// the image only neighbour border pixels, which are never extrema.  Same helpers, same operand order -> same bits.
+__host__ __device__ constexpr int det_smem_floats(int s) {
+    return (SW3 + 4 * s + 2) * (SH3 + 4 * s + 2) + 2 * (SW3 + 2 * s + 2) * (SH3 + 2 * s + 2);
+}
+
+template <int S>
+__device__ __forceinline__ void detector_response_body(const float *__restrict__ src, float *__restrict__ Lx, float *__restrict__ Ly,
+                                                       float *__restrict__ Ldet, const EvoDev &ev, int x0, int y0, float *sm,
+                                                       float thr, unsigned *__restrict__ mrow, unsigned *__restrict__ rc) {
+    constexpr int R = 2 * S + 1, RW = SW3 + 2 * R, RH = SH3 + 2 * R;          // staged Lsmooth
+    constexpr int LW = SW3 + 2 * (S + 1), LH = SH3 + 2 * (S + 1);             // Lx / Ly ring tile
+    constexpr int DW = SW3 + 2, DH = SH3 + 2;                                 // Ldet ring tile
+    constexpr int NS1 = NT / LW, BS1 = (LH + NS1 - 1) / NS1;                  // Lx / Ly tasks: LW columns x NS1 strips
+    constexpr int NS2 = NT / DW, BS2 = (DH + NS2 - 1) / NS2;                  // Ldet tasks: DW columns x NS2 strips
+    static_assert(2 * R <= 32 && DW * DH <= RW * RH, "halo fits stage_region's tail lanes; Ldet tile fits the staging buffer");
+    float *s_in = sm, *s_x = sm + RW * RH, *s_y = s_x + LW * LH;
+    float *s_d = sm;                                                          // reuses the staging buffer once Lx / Ly exist
+    const int w = ev.w, h = ev.h;
+    stage_region<R, R>(src, w, h, x0, y0, s_in);
+    __syncthreads();
+    // Strips start at min(sidx * BS, rows - BS): the last one overlaps its neighbour (both write the same values) instead of
+    // ending in guarded rows, so the unrolled loops carry no bounds branches.
+    if (threadIdx.x < LW * NS1) {   // Lx / Ly over the ring tile: ring (lr, c) is pixel (y0 - S - 1 + lr, x0 - S - 1 + c)
+        const int sidx = threadIdx.x / LW, c = threadIdx.x - sidx * LW;
+        const int r0 = min(sidx * BS1, LH - BS1);
+        const int gx = x0 - (S + 1) + c;
+        const bool xt = c > S && c <= S + SW3 && gx < w;      // a tile column inside the image
+        const int yt0 = S + 1 - r0, yt1 = min(S + SH3, h - 1 - y0 + S + 1) - r0;   // tile rows inside the image: yt0 <= o <= yt1
+        const float *col = s_in + r0 * RW + c;     // col[r * RW + {0, S, 2S}] = staged row r0 + r
+        float *ox = s_x + r0 * LW + c, *oy = s_y + r0 * LW + c;
+        int g = (y0 - (S + 1) + r0) * w + gx;
+        float hm[BS1 + 2 * S], ho[BS1 + 2 * S];
+#pragma unroll
+        for (int r = 0; r < BS1 + 2 * S; r++) {
+            const float a = col[r * RW], m = col[r * RW + S], z = col[r * RW + 2 * S];
+            hm[r] = scharr_main<S & 3>(a, z);
+            ho[r] = scharr_off<S & 3>(a, m, z, ev.norm, ev.middle);
+            if (r >= 2 * S) {
+                const int o = r - 2 * S;
+                const float vx = scharr_off<S & 3>(hm[o], hm[o + S], hm[o + 2 * S], ev.norm, ev.middle);
+                const float vy = scharr_main<S & 3>(ho[o], ho[o + 2 * S]);
+                ox[o * LW] = vx;
+                oy[o * LW] = vy;
+                if (xt && o >= yt0 && o <= yt1) {
+                    Lx[g] = vx;
+                    Ly[g] = vy;
+                }
+                g += w;
+            }
+        }
+    }
+    __syncthreads();
+    // ring rows above / below the image and ring columns left / right of it (the positions that copy are never copied from)
+    const int rt = max(0, S + 1 - y0), rb = max(0, y0 + SH3 + S + 1 - h), cl = max(0, S + 1 - x0), cr = max(0, x0 + SW3 + S + 1 - w);
+    if (rt + rb + cl + cr > 0) {      // the ring leaves the image (CTA-uniform)
+        const int nc = cl + cr, nr = LH - rt - rb;
+        for (int p = threadIdx.x; p < (rt + rb) * LW + nr * nc; p += NT) {
+            int lr, lc;
+            if (p < (rt + rb) * LW) {          // whole rows outside the image
+                const int i = p / LW;
+                lr = i < rt ? i : LH - rb + (i - rt); lc = p - i * LW;
+            } else {                           // columns outside the image of the rows inside it
+                const int i = (p - (rt + rb) * LW) / nc, j = p - (rt + rb) * LW - i * nc;
+                lr = rt + i; lc = j < cl ? j : LW - cr + (j - cl);
+            }
+            const int gy = y0 - (S + 1) + lr, gx = x0 - (S + 1) + lc;
+            const int q = (clampi(gy, 0, h - 1) - (y0 - (S + 1))) * LW + (clampi(gx, 0, w - 1) - (x0 - (S + 1)));
+            s_x[lr * LW + lc] = s_x[q];
+            s_y[lr * LW + lc] = s_y[q];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < DW * NS2) {   // Ldet over the one-pixel ring: ring (dr, c) is pixel (y0 - 1 + dr, x0 - 1 + c) = Lx ring (dr + S, c + S)
+        const int sidx = threadIdx.x / DW, c = threadIdx.x - sidx * DW;
+        const int r0 = min(sidx * BS2, DH - BS2);
+        const int gx = x0 - 1 + c;
+        const bool xt = c >= 1 && c <= SW3 && gx < w;
+        const int yt0 = 1 - r0, yt1 = min(SH3, h - y0) - r0;                 // tile rows inside the image: yt0 <= o <= yt1
+        const float *cx = s_x + r0 * LW + c, *cy = s_y + r0 * LW + c;
+        float *od = s_d + r0 * DW + c;
+        int g = (y0 - 1 + r0) * w + gx;
+        float hmx[BS2 + 2 * S], hox[BS2 + 2 * S], hoy[BS2 + 2 * S];
+#pragma unroll
+        for (int r = 0; r < BS2 + 2 * S; r++) {
+            const float a = cx[r * LW], m = cx[r * LW + S], z = cx[r * LW + 2 * S];
+            hmx[r] = scharr_main<S & 3>(a, z);                                                          // H_main(Lx)
+            hox[r] = scharr_off<S & 3>(a, m, z, ev.norm, ev.middle);                                    // H_off(Lx)
+            hoy[r] = scharr_off<S & 3>(cy[r * LW], cy[r * LW + S], cy[r * LW + 2 * S], ev.norm, ev.middle);   // H_off(Ly)
+            if (r >= 2 * S) {
+                const int o = r - 2 * S;
+                const float lxx = scharr_off<S & 3>(hmx[o], hmx[o + S], hmx[o + 2 * S], ev.norm, ev.middle);
+                const float lyy = scharr_main<S & 3>(hoy[o], hoy[o + 2 * S]);
+                const float lxy = scharr_main<S & 3>(hox[o], hox[o + 2 * S]);
+                const float v = (lxx * lyy - lxy * lxy) * ev.quat;
+                od[o * DW] = v;
+                if (xt && o >= yt0 && o <= yt1) Ldet[g] = v;
+                g += w;
+            }
+        }
+    }
+    __syncthreads();
+    // the body of k_extrema_mask on the shared Ldet tile
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const int gx = x0 + tx;
+    const bool xin = gx >= 1 && gx < w - 1;
+    const float *col = s_d + (ty * STRIP) * DW + tx;
+    const int wpr = (w + 31) >> 5;
+    float m3[STRIP + 2], sd[STRIP + 2], cn[STRIP + 2];
+#pragma unroll
+    for (int r = 0; r < STRIP + 2; r++) {
+        const float l = col[r * DW], c = col[r * DW + 1], rt = col[r * DW + 2];
+        sd[r] = fmaxf(l, rt);
+        m3[r] = fmaxf(sd[r], c);
+        cn[r] = c;
+        if (r >= 2) {
+            const int o = r - 2, gy = y0 + ty * STRIP + o;
+            const float v = cn[o + 1];
+            const float m8 = fmaxf(fmaxf(m3[o], m3[o + 2]), sd[o + 1]);
+            const bool hit = xin && gy >= 1 && gy < h - 1 && v > thr && v > m8;
+            const unsigned bits = __ballot_sync(0xffffffffu, hit);
+            if (tx == 0 && gy < h && x0 < w) {
+                mrow[(size_t)gy * wpr + (x0 >> 5)] = bits;
+                if (bits) atomicAdd(&rc[gy], (unsigned)__popc(bits));
+            }
+        }
+    }
+}
+
+// one launch per octave over the octave's tiles (tile table as k_deriv1_v3); dynamic shared memory det_smem_floats(max sigma)
+__global__ void __launch_bounds__(NT, 4) k_detector_response(const float *__restrict__ Ls, const float *__restrict__ Lt0,
+                                                             float *__restrict__ Lx, float *__restrict__ Ly, float *__restrict__ Ldet,
+                                                             size_t bstride, EvoTable T, const unsigned char *__restrict__ tile_evo,
+                                                             int tile_offset, MaskLayout ML, float thr, unsigned *__restrict__ mask,
+                                                             unsigned *__restrict__ rowcount) {
+    extern __shared__ float sm[];
+    const int gtile = blockIdx.x + tile_offset;
+    const int e = tile_evo[gtile];
+    const EvoDev ev = T.e[e];
+    int x0, y0;
+    tile_origin_v3(ev, gtile, x0, y0);
+    const size_t base = (size_t)blockIdx.z * bstride + ev.off;
+    const float *src = (e == 0 ? Lt0 : Ls) + base;   // evolution 0: Lsmooth IS Lt (lib.rs:201)
+    unsigned *mrow = mask + (size_t)blockIdx.z * ML.total_words + ML.wordbase[e];
+    unsigned *rc = rowcount + (size_t)blockIdx.z * T.total_rows + ev.rowbase;
+    switch (ev.sigma) {
+    case 1: detector_response_body<1>(src, Lx + base, Ly + base, Ldet + base, ev, x0, y0, sm, thr, mrow, rc); break;
+    case 2: detector_response_body<2>(src, Lx + base, Ly + base, Ldet + base, ev, x0, y0, sm, thr, mrow, rc); break;
+    case 3: detector_response_body<3>(src, Lx + base, Ly + base, Ldet + base, ev, x0, y0, sm, thr, mrow, rc); break;
+    case 4: detector_response_body<4>(src, Lx + base, Ly + base, Ldet + base, ev, x0, y0, sm, thr, mrow, rc); break;
+    default: detector_response_body<5>(src, Lx + base, Ly + base, Ldet + base, ev, x0, y0, sm, thr, mrow, rc); break;
+    }
+}
+
 // warp per row: expand the row's mask words into candidates at rowoff[row] (x ascending)
 __global__ void __launch_bounds__(NT) k_extrema_emit(const float *__restrict__ Ldet, size_t bstride, EvoTable T, MaskLayout ML,
                                                      const unsigned *__restrict__ mask, const unsigned *__restrict__ rowcount,
