@@ -179,3 +179,7 @@ impl TriangulatorObservations for CudaLinearEigen {
 // ---- INTEGRATION.md section 2c (include/cvb200_sfm.h) ----
 mod sfm;
 pub use sfm::*;
+
+// ---- INTEGRATION.md section 2d (include/cvb200_tri.h) ----
+mod tri;
+pub use tri::*;

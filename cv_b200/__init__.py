@@ -8,6 +8,7 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
   CameraIntrinsics(K1Distortion) <- cv-pinhole/src/lib.rs:32-240
   frame_features        <- cv-sfm VSlam::kps_descriptors        (cv-sfm/src/lib.rs:2195-2235)
+  *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
 
 There is no CPU fallback: every call runs CUDA kernels from cv_b200/libcvb200.so and raises
 CvbError when the library or a Hopper (sm_90) GPU is missing.
@@ -16,8 +17,10 @@ from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F
 from .akaze import Akaze, AkazeConfig  # noqa: F401
 from .knn import HammingHasher, LinearKnn, hamming_knn, lowe_ratio_matches, matching, symmetric_matching  # noqa: F401
 from .pinhole import CameraIntrinsics, CameraIntrinsicsK1Distortion  # noqa: F401
-from .geom import (Arrsac, EightPoint, LambdaTwist, LinearEigenTriangulator, NisterStewenius, Pcg64, Xoshiro256PlusPlus,  # noqa: F401
+from .geom import (Arrsac, EightPoint, LambdaTwist, NisterStewenius, Pcg64, Xoshiro256PlusPlus,  # noqa: F401
                    residuals_camera_to_camera, residuals_world_to_camera)
+from .triangulation import (AngularL1Triangulator, AngularLInfinityTriangulator, LinearEigenTriangulator,  # noqa: F401
+                            MeanMeanTriangulator, RelativeDltTriangulator, SineL1Triangulator)
 from .optimize import (observation_losses, single_view_simple_optimize_l2, single_view_simple_optimize_l2_batch,  # noqa: F401
                        three_view_adaptive_optimize_l2, three_view_optimize_l2_batch, three_view_simple_optimize_l2,
                        tri_landmarks_robust)

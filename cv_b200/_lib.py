@@ -1,4 +1,4 @@
-"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h)."""
+"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h)."""
 import ctypes as C
 import os
 
@@ -57,6 +57,12 @@ ABI_SYMBOLS = [
 # every symbol include/cvb200_sfm.h declares (the K1 camera and cv-sfm's frame ingestion; checked by tests/test_abi_sfm.py)
 SFM_ABI_SYMBOLS = [
     "cvb_pair_bearings_k1_dev", "cvb_two_view_pair_k1_dev", "cvb_two_view_frames_k1", "cvb_frame_features_batch", "cvb_frame_features_batch_dev",
+]
+
+# every symbol include/cvb200_tri.h declares (cv-geom's triangulators; checked by tests/test_abi_tri.py)
+TRI_ABI_SYMBOLS = [
+    "cvb_triangulator_default", "cvb_triangulate_observations", "cvb_triangulate_relative", "cvb_observation_losses_tri",
+    "cvb_tri_landmarks_robust_tri",
 ]
 
 

@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <vector>
 #include "common.cuh"
+#include "../../include/cvb200_tri.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -617,22 +618,25 @@ __device__ __noinline__ bool real_eigenvalues10(const double *Ain, double *wr, d
     return true;
 }
 
-__device__ __noinline__ bool min_right_singular_vector10(const double *Min, double eps, int max_sweeps, double *vec, double *smin) {
-    double U[FPN][FPN], V[FPN][FPN];
-    for (int i = 0; i < FPN; i++) for (int j = 0; j < FPN; j++) { U[i][j] = Min[i * FPN + j]; V[i][j] = i == j ? 1.0 : 0.0; }
+// right singular vector of the smallest singular value of an N x N matrix: one-sided Jacobi on the columns (N = 10: the five-point
+// solver; N = 4: RelativeDlt's design matrix, which is never squared into DtD)
+template <int N>
+__device__ __noinline__ bool min_right_singular_vector(const double *Min, double eps, int max_sweeps, double *vec, double *smin) {
+    double U[N][N], V[N][N];
+    for (int i = 0; i < N; i++) for (int j = 0; j < N; j++) { U[i][j] = Min[i * N + j]; V[i][j] = i == j ? 1.0 : 0.0; }
     bool converged = false;
     for (int sweep = 0; sweep < max_sweeps && !converged; sweep++) {
         converged = true;
-        for (int p = 0; p < FPN - 1; p++)
-            for (int q = p + 1; q < FPN; q++) {
+        for (int p = 0; p < N - 1; p++)
+            for (int q = p + 1; q < N; q++) {
                 double alpha = 0, beta = 0, gamma = 0;
-                for (int i = 0; i < FPN; i++) { alpha += U[i][p] * U[i][p]; beta += U[i][q] * U[i][q]; gamma += U[i][p] * U[i][q]; }
+                for (int i = 0; i < N; i++) { alpha += U[i][p] * U[i][p]; beta += U[i][q] * U[i][q]; gamma += U[i][p] * U[i][q]; }
                 if (gamma == 0.0 || fabs(gamma) <= eps * sqrt(alpha * beta)) continue;
                 converged = false;
                 const double zeta = (beta - alpha) / (2.0 * gamma);
                 const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
                 const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-                for (int i = 0; i < FPN; i++) {
+                for (int i = 0; i < N; i++) {
                     const double up = U[i][p], uq = U[i][q];
                     U[i][p] = c * up - s * uq; U[i][q] = s * up + c * uq;
                     const double vp = V[i][p], vq = V[i][q];
@@ -642,12 +646,12 @@ __device__ __noinline__ bool min_right_singular_vector10(const double *Min, doub
     }
     if (!converged) return false;
     int best = 0; double bn = -1.0;
-    for (int j = 0; j < FPN; j++) {
-        double nn = 0; for (int i = 0; i < FPN; i++) nn += U[i][j] * U[i][j];
+    for (int j = 0; j < N; j++) {
+        double nn = 0; for (int i = 0; i < N; i++) nn += U[i][j] * U[i][j];
         if (bn < 0.0 || nn < bn) { bn = nn; best = j; }
     }
     *smin = sqrt(bn);
-    for (int i = 0; i < FPN; i++) vec[i] = V[i][best];
+    for (int i = 0; i < N; i++) vec[i] = V[i][best];
     return true;
 }
 
@@ -768,7 +772,7 @@ __device__ int five_point(const double *a, const double *b, const uint32_t *idx,
         double vec[10], smin;
         for (int k = 0; k < 100; k++) Mx[k] = At[k];
         for (int k = 0; k < 10; k++) Mx[k * 10 + k] -= wr[i];
-        if (!min_right_singular_vector10(Mx, 1e-15, 1000, vec, &smin)) continue;
+        if (!min_right_singular_vector<FPN>(Mx, 1e-15, 1000, vec, &smin)) continue;
         if (!(smin < 1e-12)) continue;
         double ev[9], E[9];
         for (int r = 0; r < 9; r++) ev[r] = eb[r][0] * vec[row0] + eb[r][1] * vec[row0 + 1] + eb[r][2] * vec[row0 + 2] + eb[r][3] * vec[row0 + 3];
@@ -820,13 +824,14 @@ __global__ void __launch_bounds__(256) k_residuals(const cvb_pose *__restrict__ 
     }
 }
 
-// cv-geom/src/triangulation.rs:82-130: n >= 2 observations (WorldToCamera pose, bearing) -> homogeneous world point
-__device__ bool triangulate_linear_eigen(const cvb_pose *poses, const double *bearings, uint32_t n, double *p) {
+// cv-geom/src/triangulation.rs:82-130: n >= 2 observations (WorldToCamera pose, bearing) -> homogeneous world point;
+// eps / max_sweeps: the triangulator's epsilon / max_iterations (Default 1e-12 / 1000) handed to try_symmetric_eigen
+__device__ bool triangulate_linear_eigen(const cvb_pose *poses, const double *bearings, uint32_t n, double *p, double eps, int max_sweeps) {
     if (n < 2) return false;
     double A[16], d[4], V[16];
     for (int i = 0; i < 16; i++) A[i] = 0.0;
     for (uint32_t i = 0; i < n; i++) design_add(poses[i].r, poses[i].t, bearings + 3 * (size_t)i, A);
-    if (!sym_eigen<4>(A, 1e-12, 1000, d, V)) return false;
+    if (!sym_eigen<4>(A, eps, max_sweeps, d, V)) return false;
     int best = 0;
     for (int i = 1; i < 4; i++)
         if (d[i] < d[best]) best = i;
@@ -840,18 +845,6 @@ __device__ bool triangulate_linear_eigen(const cvb_pose *poses, const double *be
         if (signbit(dot3(wb, p))) return false;
     }
     return true;
-}
-// one thread per landmark
-__global__ void __launch_bounds__(128) k_triangulate(const cvb_pose *__restrict__ poses, const double *__restrict__ bearings,
-                                                     const uint32_t *__restrict__ offsets, uint32_t L, double *__restrict__ xyzw,
-                                                     uint8_t *__restrict__ ok) {
-    const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
-    if (l >= L) return;
-    const uint32_t o0 = offsets[l], o1 = offsets[l + 1];
-    double p[4] = {0, 0, 0, 0};
-    const bool good = triangulate_linear_eigen(poses + o0, bearings + 3 * (size_t)o0, o1 - o0, p);
-    ok[l] = good ? 1 : 0;
-    for (int i = 0; i < 4; i++) xyzw[(size_t)l * 4 + i] = good ? p[i] : 0.0;
 }
 
 // cv-sfm keeps calibrated bearings per feature (CameraModel::calibrate, cv-pinhole/src/lib.rs:108-116, on
@@ -1135,9 +1128,206 @@ __device__ double transformed_cosine_distance(const cvb_pose &P, const double *p
     from_homogeneous(q);
     return 1.0 - dot3(q, bearing);
 }
-// cv-sfm/src/lib.rs:2570-2620 observation_loss of every observation; one thread per landmark
-__global__ void __launch_bounds__(128) k_observation_losses(const cvb_pose *__restrict__ poses, const double *__restrict__ bearings,
-                                                            const uint32_t *__restrict__ offsets, uint32_t L, double *__restrict__ loss) {
+// ---- the triangulators of cv-geom/src/triangulation.rs (include/cvb200_tri.h), each restated on the checker's side as well
+// (ref_triangulation.c).  Reference details kept as they are:
+//  - Isometry x unit vector applies the rotation only (nalgebra): a world-frame bearing is R^T b, a camera centre R^T (-t).
+//  - The cheirality tests use the sign bit (is_sign_positive): a dot product of -0.0 fails.
+__device__ __forceinline__ void rotTv(const double *R, const double *v, double *o) {
+    for (int c = 0; c < 3; c++) o[c] = R[c] * v[0] + R[3 + c] * v[1] + R[6 + c] * v[2];
+}
+// camera centre and world-frame bearing of one (WorldToCamera, bearing) observation: pose.inverse().isometry() applied to both
+__device__ __forceinline__ void obs_world(const cvb_pose &P, const double *b, double *centre, double *wb) {
+    const double nt[3] = {-P.t[0], -P.t[1], -P.t[2]};
+    rotTv(P.r, nt, centre);
+    rotTv(P.r, b, wb);
+}
+__device__ __forceinline__ bool finite4(const double *p) { return isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]) && isfinite(p[3]); }
+// max_iterations (usize upstream) as the Jacobi sweep bound
+__device__ __forceinline__ int tri_sweeps(const cvb_triangulator &T) { return T.max_iterations > 0x7fffffffu ? 0x7fffffff : (int)T.max_iterations; }
+
+// cv-geom/src/triangulation.rs:228-276 SineL1Triangulator.  Kept from the reference:
+//  - when LinearEigen's point has w == 0 (point() is None) that point is returned unrefined (:240-244);
+//  - scale = optimization_rate / count (:246), and the loop stops when |delta|^2 / |p|^2 < epsilon^2 (:269);
+//  - after the refinement there is NO finiteness or cheirality check (:274);
+//  - Default is epsilon 1e-12, 1000 iterations, rate 1.0, although the setter's doc comment says 0.01 (:197-199, :218-226).
+// W (6 doubles per observation) receives every observation's camera centre and world-frame bearing once, before the loop; the
+// reference recomputes them every iteration with the same expressions, so the bits are the same.  The gradients are summed in
+// observation order, starting from zero, as the reference's `.sum()` does.
+__device__ bool triangulate_sine_l1(const cvb_triangulator &T, const cvb_pose *P, const double *B, uint32_t n, double *W, double *p) {
+    if (!triangulate_linear_eigen(P, B, n, p, T.epsilon, tri_sweeps(T))) return false;
+    if (p[3] == 0.0) return true;
+    double x[3] = {p[0] / p[3], p[1] / p[3], p[2] / p[3]};
+    for (uint32_t i = 0; i < n; i++) obs_world(P[i], B + 3 * (size_t)i, W + 6 * (size_t)i, W + 6 * (size_t)i + 3);
+    const double scale = T.optimization_rate / (double)n, eps2 = T.epsilon * T.epsilon;
+    for (uint32_t it = 0; it < T.max_iterations; it++) {
+        double s[3] = {0.0, 0.0, 0.0};
+        for (uint32_t i = 0; i < n; i++) {
+            const double *c = W + 6 * (size_t)i, *wb = c + 3;
+            const double tr[3] = {c[0] - x[0], c[1] - x[1], c[2] - x[2]};
+            const double d = dot3(tr, wb);
+            for (int k = 0; k < 3; k++) s[k] = s[k] + (tr[k] - d * wb[k]);   // epipolar::point_gradient (epipolar.rs:174-179)
+        }
+        const double delta[3] = {scale * s[0], scale * s[1], scale * s[2]};
+        for (int k = 0; k < 3; k++) x[k] = x[k] + delta[k];
+        if (dot3(delta, delta) / dot3(x, x) < eps2) break;
+    }
+    p[0] = x[0]; p[1] = x[1]; p[2] = x[2]; p[3] = 1.0;
+    from_homogeneous(p);   // Projective::from_point
+    return true;
+}
+
+// cv-geom/src/triangulation.rs:392-442 MeanMeanTriangulator.  For n <= 1 it divides by zero (0 / 0, or a zero projection distance)
+// and the finiteness filter returns None, as in the reference; nothing beyond the n observations is read.
+__device__ bool triangulate_mean_mean(const cvb_pose *P, const double *B, uint32_t n, double *p) {
+    const double total = (double)n;
+    double sc[3] = {0.0, 0.0, 0.0}, sb[3] = {0.0, 0.0, 0.0}, c[3], wb[3];
+    for (uint32_t i = 0; i < n; i++) {
+        obs_world(P[i], B + 3 * (size_t)i, c, wb);
+        for (int k = 0; k < 3; k++) { sc[k] = sc[k] + c[k]; sb[k] = sb[k] + wb[k]; }
+    }
+    const double ac[3] = {sc[0] / total, sc[1] / total, sc[2] / total};
+    const double nb = norm3(sb);
+    const double ab[3] = {sb[0] / nb, sb[1] / nb, sb[2] / nb};
+    double sum = 0.0;
+    for (uint32_t i = 0; i < n; i++) {
+        obs_world(P[i], B + 3 * (size_t)i, c, wb);
+        const double trans[3] = {ac[0] - c[0], ac[1] - c[1], ac[2] - c[2]};
+        double q[3], bt[3];
+        cross3(ab, wb, q);
+        const double r = 1.0 / dot3(q, q);
+        const double qs[3] = {q[0] * r, q[1] * r, q[2] * r};
+        cross3(wb, trans, bt);
+        sum = sum + dot3(qs, bt);
+    }
+    const double w = 1.0 / (sum / total);
+    p[0] = ab[0] + ac[0] * w; p[1] = ab[1] + ac[1] * w; p[2] = ab[2] + ac[2] * w; p[3] = w;
+    from_homogeneous(p);
+    if (!finite4(p)) return false;
+    for (uint32_t i = 0; i < n; i++) {
+        obs_world(P[i], B + 3 * (size_t)i, c, wb);
+        if (signbit(dot3(wb, p))) return false;
+    }
+    return true;
+}
+
+// TriangulatorObservations (methods 0-2; the host rejects the others).  W: SineL1's scratch, 6 doubles per observation.
+__device__ bool triangulate_observations(const cvb_triangulator &T, const cvb_pose *P, const double *B, uint32_t n, double *W, double *p) {
+    switch (T.method) {
+    case CVB_TRI_SINE_L1: return triangulate_sine_l1(T, P, B, n, W, p);
+    case CVB_TRI_MEAN_MEAN: return triangulate_mean_mean(P, B, n, p);
+    default: return triangulate_linear_eigen(P, B, n, p, T.epsilon, tri_sweeps(T));
+    }
+}
+// one thread per landmark
+__global__ void __launch_bounds__(128) k_triangulate(cvb_triangulator T, const cvb_pose *__restrict__ poses, const double *__restrict__ bearings,
+                                                     const uint32_t *__restrict__ offsets, uint32_t L, double *__restrict__ W,
+                                                     double *__restrict__ xyzw, uint8_t *__restrict__ ok) {
+    const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
+    if (l >= L) return;
+    const uint32_t o0 = offsets[l], o1 = offsets[l + 1];
+    double p[4] = {0, 0, 0, 0};
+    const bool good = triangulate_observations(T, poses + o0, bearings + 3 * (size_t)o0, o1 - o0, W ? W + 6 * (size_t)o0 : nullptr, p);
+    ok[l] = good ? 1 : 0;
+    for (int i = 0; i < 4; i++) xyzw[(size_t)l * 4 + i] = good ? p[i] : 0.0;
+}
+
+// TriangulatorRelative of methods 0-2 is the blanket impl (cv-core/src/triangulation.rs:21-35, 52-67): the observations
+// [(identity, a), (pose, b)], then CameraPoint::from_homogeneous once more (which can change the last bit)
+__device__ bool triangulate_relative_obs(const cvb_triangulator &T, const cvb_pose &P, const double *a, const double *b, double *p) {
+    cvb_pose O[2];
+    for (int k = 0; k < 9; k++) O[0].r[k] = (k % 4 == 0) ? 1.0 : 0.0;
+    O[0].t[0] = O[0].t[1] = O[0].t[2] = 0.0;
+    O[1] = P;
+    const double B[6] = {a[0], a[1], a[2], b[0], b[1], b[2]};
+    double W[12];
+    if (!triangulate_observations(T, O, B, 2, W, p)) return false;
+    from_homogeneous(p);
+    return true;
+}
+// cv-geom/src/triangulation.rs:322-363 RelativeDltTriangulator.  nalgebra's try_svd (not in the reference checkout) is restated as
+// one-sided Jacobi on the 4x4 design matrix itself -- the right singular vector of the smallest singular value -- never as the
+// eigenvectors of DtD, which squares the condition number and loses the null vector at low parallax.  epsilon / max_iterations bound
+// the Jacobi sweeps as they bound the eigen restatements'.  Default is 1e-12 / 1000 although the doc comments say 1e-9 / 100 (:293-320).
+__device__ bool triangulate_relative_dlt(const cvb_triangulator &T, const cvb_pose &P, const double *a, const double *b, double *p) {
+    const double D[16] = {-a[2], 0.0, a[0], 0.0,
+                          0.0, -a[2], a[1], 0.0,
+                          b[0] * P.r[6] - b[2] * P.r[0], b[0] * P.r[7] - b[2] * P.r[1], b[0] * P.r[8] - b[2] * P.r[2], b[0] * P.t[2] - b[2] * P.t[0],
+                          b[1] * P.r[6] - b[2] * P.r[3], b[1] * P.r[7] - b[2] * P.r[4], b[1] * P.r[8] - b[2] * P.r[5], b[1] * P.t[2] - b[2] * P.t[1]};
+    double smin;
+    if (!min_right_singular_vector<4>(D, T.epsilon, tri_sweeps(T), p, &smin)) return false;
+    from_homogeneous(p);
+    if (!finite4(p)) return false;
+    double bw[3];
+    rotTv(P.r, b, bw);
+    return !signbit(dot3(p, a)) && !signbit(dot3(p, bw));
+}
+// cv-geom/src/triangulation.rs:472-530 AngularL1Triangulator (linf = false) and :558-606 AngularLInfinityTriangulator (linf = true).
+// Both invert the relative pose and swap a and b first (:483-487, :569-573) and build the point on the (corrected) swapped b.
+// AngularL1 forms z = b x a; epipolar.rs's sine-L1 point forms a x b, so the two are not shared.
+__device__ bool triangulate_angular(bool linf, const cvb_pose &P, const double *a_in, const double *b_in, double *p) {
+    const double mt[3] = {-P.t[0], -P.t[1], -P.t[2]};
+    // after the swap: b is the old a, a the old b carried by the inverse rotation, t the inverse pose's translation
+    double t[3], a[3], b[3] = {a_in[0], a_in[1], a_in[2]};
+    rotTv(P.r, mt, t);
+    rotTv(P.r, b_in, a);
+    const double tn = norm3(t);
+    const double nt[3] = {t[0] / tn, t[1] / tn, t[2] / tn};
+    if (!linf) {
+        double ca[3], cb[3], v[3];
+        cross3(a, nt, ca); cross3(b, nt, cb);
+        const double can = norm3(ca), cbn = norm3(cb);
+        if (can < cbn) {   // algorithm 12: correct a
+            const double nb[3] = {cb[0] / cbn, cb[1] / cbn, cb[2] / cbn}, d = dot3(a, nb);
+            for (int k = 0; k < 3; k++) v[k] = a[k] - d * nb[k];
+            normalize3(v, a);
+        } else {           // algorithm 13: correct b
+            const double na[3] = {ca[0] / can, ca[1] / can, ca[2] / can}, d = dot3(b, na);
+            for (int k = 0; k < 3; k++) v[k] = b[k] - d * na[k];
+            normalize3(v, b);
+        }
+    } else {
+        const double sp[3] = {a[0] + b[0], a[1] + b[1], a[2] + b[2]}, sm[3] = {a[0] - b[0], a[1] - b[1], a[2] - b[2]};
+        double na[3], nb[3], n[3], va[3], vb[3];
+        cross3(sp, nt, na); cross3(sm, nt, nb);
+        const double nas = dot3(na, na), nbs = dot3(nb, nb);
+        if (nas > nbs) { const double s = sqrt(nas); n[0] = na[0] / s; n[1] = na[1] / s; n[2] = na[2] / s; }
+        else { const double s = sqrt(nbs); n[0] = nb[0] / s; n[1] = nb[1] / s; n[2] = nb[2] / s; }
+        const double da = dot3(a, n), db = dot3(b, n);
+        for (int k = 0; k < 3; k++) { va[k] = a[k] - da * n[k]; vb[k] = b[k] - db * n[k]; }
+        normalize3(va, a); normalize3(vb, b);
+    }
+    double z[3], ta[3];
+    cross3(b, a, z); cross3(t, a, ta);
+    p[0] = b[0]; p[1] = b[1]; p[2] = b[2]; p[3] = dot3(z, z) / dot3(z, ta);
+    from_homogeneous(p);
+    if (!finite4(p)) return false;
+    return !signbit(dot3(p, a)) && !signbit(dot3(p, b));
+}
+// one thread per (relative pose, a, b) triple; npose = 1 shares poses[0]
+__global__ void __launch_bounds__(128) k_triangulate_relative(cvb_triangulator T, const cvb_pose *__restrict__ poses, uint32_t npose,
+                                                              const double *__restrict__ a, const double *__restrict__ b, uint32_t n,
+                                                              double *__restrict__ xyzw, uint8_t *__restrict__ ok) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const cvb_pose P = poses[npose == 1 ? 0 : i];
+    const double *ai = a + 3 * (size_t)i, *bi = b + 3 * (size_t)i;
+    double p[4] = {0, 0, 0, 0};
+    bool good;
+    switch (T.method) {
+    case CVB_TRI_RELATIVE_DLT: good = triangulate_relative_dlt(T, P, ai, bi, p); break;
+    case CVB_TRI_ANGULAR_L1: good = triangulate_angular(false, P, ai, bi, p); break;
+    case CVB_TRI_ANGULAR_LINF: good = triangulate_angular(true, P, ai, bi, p); break;
+    default: good = triangulate_relative_obs(T, P, ai, bi, p);
+    }
+    ok[i] = good ? 1 : 0;
+    for (int k = 0; k < 4; k++) xyzw[(size_t)i * 4 + k] = good ? p[k] : 0.0;
+}
+
+// cv-sfm/src/lib.rs:2570-2620 observation_loss of every observation; one thread per landmark.  The landmarks of three or more
+// observations go through the triangulator T (self.triangulator upstream); W: SineL1's scratch, 6 doubles per observation.
+__global__ void __launch_bounds__(128) k_observation_losses(cvb_triangulator T, const cvb_pose *__restrict__ poses, const double *__restrict__ bearings,
+                                                            const uint32_t *__restrict__ offsets, uint32_t L, double *__restrict__ W,
+                                                            double *__restrict__ loss) {
     const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= L) return;
     const uint32_t o0 = offsets[l], n = offsets[l + 1] - o0;
@@ -1155,12 +1345,13 @@ __global__ void __launch_bounds__(128) k_observation_losses(const cvb_pose *__re
         return;
     }
     double p[4];
-    const bool ok = triangulate_linear_eigen(P, B, n, p);
+    const bool ok = triangulate_observations(T, P, B, n, W ? W + 6 * (size_t)o0 : nullptr, p);
     for (uint32_t i = 0; i < n; i++) loss[o0 + i] = ok ? transformed_cosine_distance(P[i], p, B + 3 * (size_t)i) : 2.0;
 }
-// cv-sfm/src/lib.rs:1320-1360 is_tri_landmark_robust; one thread per (centre, first, second) observation triple of one pose pair
-__global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_pose first, cvb_pose second, const double *__restrict__ obs, uint32_t n,
-                                                             double max_cos, double inc_min_cos, uint8_t *__restrict__ out) {
+// cv-sfm/src/lib.rs:1320-1360 is_tri_landmark_robust with the triangulator T; one thread per (centre, first, second) observation
+// triple of one pose pair
+__global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T, cvb_pose first, cvb_pose second, const double *__restrict__ obs,
+                                                             uint32_t n, double max_cos, double inc_min_cos, uint8_t *__restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const double *c = obs + 9 * (size_t)i, *f = c + 3, *s = c + 6;
@@ -1168,8 +1359,8 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_pose first, cvb
     for (int k = 0; k < 9; k++) P[0].r[k] = (k % 4 == 0) ? 1.0 : 0.0;
     P[0].t[0] = P[0].t[1] = P[0].t[2] = 0.0;
     P[1] = first; P[2] = second;
-    double p[4];
-    if (!triangulate_linear_eigen(P, c, 3, p)) { out[i] = 0; return; }
+    double p[4], W[18];
+    if (!triangulate_observations(T, P, c, 3, W, p)) { out[i] = 0; return; }
     from_homogeneous(p);   // CameraPoint::from_homogeneous(p.0)
     double fc[3], sc[3];
     for (int k = 0; k < 3; k++) {
@@ -1984,32 +2175,106 @@ int cvb_residuals_world_to_camera(cvb_ctx *ctx, const cvb_pose *poses, uint32_t 
     return residuals_host(ctx, 1, poses, m, bearings, world, n, out);
 }
 
-int cvb_triangulate_linear_eigen(cvb_ctx *ctx, const cvb_pose *poses, const double *bearings, const uint32_t *offsets, uint32_t L,
-                                 double *xyzw_out, uint8_t *ok_out) {
-    if (!ctx) return CVB_EINVAL;
-    if (L == 0) return 0;
-    if (!poses || !bearings || !offsets || !xyzw_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+// ---- include/cvb200_tri.h --------------------------------------------------------------------------------------------------
+void cvb_triangulator_default(cvb_triangulator *t, int32_t method) {
+    if (!t) return;
+    memset(t, 0, sizeof(*t));
+    t->method = method;
+    switch (method) {
+    case CVB_TRI_LINEAR_EIGEN: case CVB_TRI_RELATIVE_DLT: t->epsilon = 1e-12; t->max_iterations = 1000; break;
+    case CVB_TRI_SINE_L1: t->epsilon = 1e-12; t->max_iterations = 1000; t->optimization_rate = 1.0; break;
+    default: break;   // MeanMean, AngularL1, AngularLInfinity have no settings
+    }
+}
+
+// the triangulator must be one of the six methods, and one of the TriangulatorObservations (0-2) unless `relative`
+static int tri_check(cvb_ctx *ctx, const cvb_triangulator *tri, bool relative) {
+    if (!tri) return cvb_set_error(ctx, CVB_EINVAL, "null triangulator");
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_ANGULAR_LINF)
+        return cvb_set_error(ctx, CVB_EINVAL, "unknown triangulator method %d", tri->method);
+    if (!relative && tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, CVB_EINVAL, "triangulator method %d is TriangulatorRelative only", tri->method);
+    return 0;
+}
+static int offsets_check(cvb_ctx *ctx, const uint32_t *offsets, uint32_t L) {
     for (uint32_t l = 0; l < L; l++)
         if (offsets[l + 1] < offsets[l]) return cvb_set_error(ctx, CVB_EINVAL, "offsets must be non-decreasing");
+    return 0;
+}
+// SineL1's per-observation scratch (camera centre, world-frame bearing) in the workspace buffer `b`, which the observation entry
+// points do not otherwise use; null for the other methods
+static int sine_l1_scratch(cvb_ctx *ctx, GeomWorkspace *g, const cvb_triangulator *tri, uint32_t nobs, double **W) {
+    *W = nullptr;
+    if (tri->method != CVB_TRI_SINE_L1) return 0;
+    int rc = g->b.ensure(ctx, sizeof(double) * 6 * (size_t)nobs);
+    if (rc) return rc;
+    *W = (double *)g->b.p;
+    return 0;
+}
+
+int cvb_triangulate_observations(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses, const double *bearings,
+                                 const uint32_t *offsets, uint32_t L, double *xyzw_out, uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, false))) return rc;
+    if (L == 0) return 0;
+    if (!poses || !bearings || !offsets || !xyzw_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((rc = offsets_check(ctx, offsets, L))) return rc;
     const uint32_t nobs = offsets[L];
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     GeomWorkspace *g = gws(ctx);
-    int rc;
+    double *W;
     if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * (size_t)nobs))) return rc;
     if ((rc = upload(ctx, g->a, bearings, sizeof(double) * 3 * (size_t)nobs))) return rc;
     if ((rc = upload(ctx, g->offsets, offsets, sizeof(uint32_t) * ((size_t)L + 1)))) return rc;
     if ((rc = g->out.ensure(ctx, sizeof(double) * 4 * (size_t)L))) return rc;
     if ((rc = g->ok.ensure(ctx, L))) return rc;
+    if ((rc = sine_l1_scratch(ctx, g, tri, nobs, &W))) return rc;
     {
         CVB_PROF(ctx, "k_triangulate", 120.0 * nobs);
-        k_triangulate<<<cdiv(L, 128), 128, 0, ctx->stream>>>((const cvb_pose *)g->poses.p, (const double *)g->a.p, (const uint32_t *)g->offsets.p, L,
-                                                             (double *)g->out.p, (uint8_t *)g->ok.p);
+        k_triangulate<<<cdiv(L, 128), 128, 0, ctx->stream>>>(*tri, (const cvb_pose *)g->poses.p, (const double *)g->a.p, (const uint32_t *)g->offsets.p,
+                                                             L, W, (double *)g->out.p, (uint8_t *)g->ok.p);
         CVB_LAUNCH_CHECK(ctx);
     }
     CVB_CUDA(ctx, cudaMemcpyAsync(xyzw_out, g->out.p, sizeof(double) * 4 * (size_t)L, cudaMemcpyDeviceToHost, ctx->stream));
     CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, L, cudaMemcpyDeviceToHost, ctx->stream));
     CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
     return 0;
+}
+
+int cvb_triangulate_relative(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses, uint32_t npose, const double *a,
+                             const double *b, uint32_t n, double *xyzw_out, uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, true))) return rc;
+    if (n == 0) return 0;
+    if (npose != 1 && npose != n) return cvb_set_error(ctx, CVB_EINVAL, "npose must be 1 or n (%u), not %u", n, npose);
+    if (!poses || !a || !b || !xyzw_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * (size_t)npose))) return rc;
+    if ((rc = upload(ctx, g->a, a, sizeof(double) * 3 * (size_t)n))) return rc;
+    if ((rc = upload(ctx, g->b, b, sizeof(double) * 3 * (size_t)n))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * 4 * (size_t)n))) return rc;
+    if ((rc = g->ok.ensure(ctx, n))) return rc;
+    {
+        CVB_PROF(ctx, "k_triangulate_relative", 56.0 * n + sizeof(cvb_pose) * (double)npose);
+        k_triangulate_relative<<<cdiv(n, 128), 128, 0, ctx->stream>>>(*tri, (const cvb_pose *)g->poses.p, npose, (const double *)g->a.p,
+                                                                      (const double *)g->b.p, n, (double *)g->out.p, (uint8_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(xyzw_out, g->out.p, sizeof(double) * 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, n, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+// LinearEigenTriangulator::default() through the observations entry point (one kernel for every observations triangulator)
+int cvb_triangulate_linear_eigen(cvb_ctx *ctx, const cvb_pose *poses, const double *bearings, const uint32_t *offsets, uint32_t L,
+                                 double *xyzw_out, uint8_t *ok_out) {
+    cvb_triangulator t;
+    cvb_triangulator_default(&t, CVB_TRI_LINEAR_EIGEN);
+    return cvb_triangulate_observations(ctx, &t, poses, bearings, offsets, L, xyzw_out, ok_out);
 }
 
 int cvb_arrsac_eight_point(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, const double *a, const double *b, uint32_t n, cvb_rng *rng,
@@ -2148,52 +2413,69 @@ int cvb_three_view_optimize_l2(cvb_ctx *ctx, const cvb_pose *poses, uint32_t B, 
     return download_poses_updates(ctx, g, poses_out, 2 * (size_t)B, updates_out, B);
 }
 
-int cvb_observation_losses(cvb_ctx *ctx, const cvb_pose *poses, const double *bearings, const uint32_t *offsets, uint32_t L,
-                           double *loss_out) {
+int cvb_observation_losses_tri(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses, const double *bearings,
+                               const uint32_t *offsets, uint32_t L, double *loss_out) {
     if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, false))) return rc;
     if (L == 0) return 0;
     if (!poses || !bearings || !offsets || !loss_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
-    for (uint32_t l = 0; l < L; l++)
-        if (offsets[l + 1] < offsets[l]) return cvb_set_error(ctx, CVB_EINVAL, "offsets must be non-decreasing");
+    if ((rc = offsets_check(ctx, offsets, L))) return rc;
     const uint32_t nobs = offsets[L];
     if (nobs == 0) return 0;
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     GeomWorkspace *g = gws(ctx);
-    int rc;
+    double *W;
     if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * (size_t)nobs))) return rc;
     if ((rc = upload(ctx, g->a, bearings, sizeof(double) * 3 * (size_t)nobs))) return rc;
     if ((rc = upload(ctx, g->offsets, offsets, sizeof(uint32_t) * ((size_t)L + 1)))) return rc;
     if ((rc = g->out.ensure(ctx, sizeof(double) * (size_t)nobs))) return rc;
+    if ((rc = sine_l1_scratch(ctx, g, tri, nobs, &W))) return rc;
     {
         CVB_PROF(ctx, "k_observation_losses", 128.0 * nobs);
-        k_observation_losses<<<cdiv(L, 128), 128, 0, ctx->stream>>>((const cvb_pose *)g->poses.p, (const double *)g->a.p,
-                                                                    (const uint32_t *)g->offsets.p, L, (double *)g->out.p);
+        k_observation_losses<<<cdiv(L, 128), 128, 0, ctx->stream>>>(*tri, (const cvb_pose *)g->poses.p, (const double *)g->a.p,
+                                                                    (const uint32_t *)g->offsets.p, L, W, (double *)g->out.p);
         CVB_LAUNCH_CHECK(ctx);
     }
     CVB_CUDA(ctx, cudaMemcpyAsync(loss_out, g->out.p, sizeof(double) * (size_t)nobs, cudaMemcpyDeviceToHost, ctx->stream));
     CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
     return 0;
 }
+int cvb_observation_losses(cvb_ctx *ctx, const cvb_pose *poses, const double *bearings, const uint32_t *offsets, uint32_t L,
+                           double *loss_out) {
+    cvb_triangulator t;
+    cvb_triangulator_default(&t, CVB_TRI_LINEAR_EIGEN);
+    return cvb_observation_losses_tri(ctx, &t, poses, bearings, offsets, L, loss_out);
+}
 
-int cvb_tri_landmarks_robust(cvb_ctx *ctx, const cvb_pose *first_pose, const cvb_pose *second_pose, const double *observations, uint32_t n,
-                             double maximum_cosine_distance, double incidence_minimum_cosine_distance, uint8_t *robust_out) {
+int cvb_tri_landmarks_robust_tri(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *first_pose, const cvb_pose *second_pose,
+                                 const double *observations, uint32_t n, double maximum_cosine_distance,
+                                 double incidence_minimum_cosine_distance, uint8_t *robust_out) {
     if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, false))) return rc;
     if (n == 0) return 0;
     if (!first_pose || !second_pose || !observations || !robust_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     GeomWorkspace *g = gws(ctx);
-    int rc;
     if ((rc = upload(ctx, g->a, observations, sizeof(double) * 9 * (size_t)n))) return rc;
     if ((rc = g->ok.ensure(ctx, n))) return rc;
     {
         CVB_PROF(ctx, "k_tri_landmark_robust", 72.0 * n);
-        k_tri_landmark_robust<<<cdiv(n, 128), 128, 0, ctx->stream>>>(*first_pose, *second_pose, (const double *)g->a.p, n, maximum_cosine_distance,
-                                                                     incidence_minimum_cosine_distance, (uint8_t *)g->ok.p);
+        k_tri_landmark_robust<<<cdiv(n, 128), 128, 0, ctx->stream>>>(*tri, *first_pose, *second_pose, (const double *)g->a.p, n,
+                                                                     maximum_cosine_distance, incidence_minimum_cosine_distance, (uint8_t *)g->ok.p);
         CVB_LAUNCH_CHECK(ctx);
     }
     CVB_CUDA(ctx, cudaMemcpyAsync(robust_out, g->ok.p, n, cudaMemcpyDeviceToHost, ctx->stream));
     CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
     return 0;
+}
+int cvb_tri_landmarks_robust(cvb_ctx *ctx, const cvb_pose *first_pose, const cvb_pose *second_pose, const double *observations, uint32_t n,
+                             double maximum_cosine_distance, double incidence_minimum_cosine_distance, uint8_t *robust_out) {
+    cvb_triangulator t;
+    cvb_triangulator_default(&t, CVB_TRI_LINEAR_EIGEN);
+    return cvb_tri_landmarks_robust_tri(ctx, &t, first_pose, second_pose, observations, n, maximum_cosine_distance,
+                                        incidence_minimum_cosine_distance, robust_out);
 }
 
 }  // extern "C"

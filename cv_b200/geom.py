@@ -4,7 +4,7 @@
       (eight-point/src/lib.rs:70-84, lambda-twist/src/lib.rs:330-347), batched over many minimal samples
   residuals_camera_to_camera / _world_to_camera <- sample_consensus::Model::residual
       (cv-core/src/pose.rs:249-296, 194-202)
-  LinearEigenTriangulator.triangulate_observations <- cv-geom/src/triangulation.rs:82-130
+  LinearEigenTriangulator and cv-geom's other triangulators: cv_b200/triangulation.py
   Arrsac.model / model_inliers                  <- arrsac::Arrsac as sample_consensus::Consensus
       (call sites akaze/tests/estimate_pose.rs:63-67, lambda-twist/tests/consensus.rs:20,59-61)
   Xoshiro256PlusPlus / Pcg64                     <- rand_xoshiro / rand_pcg generators handed to Arrsac::new
@@ -77,7 +77,6 @@ def _lib(ctx):
                                             C.POINTER(u32), C.POINTER(C.c_int32)]
         L.cvb_residuals_camera_to_camera.argtypes = [vp, vp, u32, vp, vp, u32, vp]
         L.cvb_residuals_world_to_camera.argtypes = [vp, vp, u32, vp, vp, u32, vp]
-        L.cvb_triangulate_linear_eigen.argtypes = [vp, vp, vp, vp, u32, vp, vp]
         L.cvb_arrsac_eight_point.argtypes = [vp, C.POINTER(ArrsacCfg), vp, vp, u32, C.POINTER(Rng), C.POINTER(Pose), vp, u32,
                                              C.POINTER(u32), C.POINTER(C.c_int32)]
         L.cvb_arrsac_p3p.argtypes = L.cvb_arrsac_eight_point.argtypes
@@ -191,28 +190,6 @@ def residuals_world_to_camera(poses, bearings, world, ctx=None):
     out = np.zeros((len(p), len(a)), np.float64)
     ctx.check(L.cvb_residuals_world_to_camera(ctx.handle, p.ctypes.data, len(p), a.ctypes.data, b.ctypes.data, len(a), out.ctypes.data))
     return out
-
-
-class LinearEigenTriangulator:
-    """cv_geom::triangulation::LinearEigenTriangulator (TriangulatorObservations), batched over landmarks."""
-
-    def triangulate_batch(self, poses, bearings, offsets, ctx=None):
-        ctx, L = _lib(ctx)
-        p = _poses_in(poses); b = _f64(bearings, 3)
-        off = np.ascontiguousarray(offsets, np.uint32)
-        _same_len(p, b, "poses, bearings")
-        if len(off) < 1 or off[0] != 0 or (np.diff(off.astype(np.int64)) < 0).any() or off[-1] > len(p):
-            raise ValueError("offsets must start at 0, be non-decreasing and end within the observations")
-        nl = len(off) - 1
-        out = np.zeros((nl, 4), np.float64); ok = np.zeros(nl, np.uint8)
-        ctx.check(L.cvb_triangulate_linear_eigen(ctx.handle, p.ctypes.data, b.ctypes.data, off.ctypes.data, nl, out.ctypes.data, ok.ctypes.data))
-        return out, ok.astype(bool)
-
-    def triangulate_observations(self, pairs, ctx=None):
-        """pairs: [((R, t), bearing), ...] -> homogeneous WorldPoint or None"""
-        poses = [p for p, _ in pairs]
-        out, ok = self.triangulate_batch(poses, np.array([b for _, b in pairs], np.float64).reshape(-1, 3), [0, len(pairs)], ctx)
-        return out[0] if ok[0] else None
 
 
 class Arrsac:

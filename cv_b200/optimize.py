@@ -15,6 +15,7 @@ import numpy as np
 
 from ._lib import default_context
 from .geom import POSE_DTYPE, _f64, _poses_in
+from .triangulation import _lib as _tri_lib
 
 
 def _lib(ctx):
@@ -86,22 +87,36 @@ def three_view_adaptive_optimize_l2(poses, iterations, landmarks, ctx=None):
     return three_view_optimize_l2_batch([poses], 0.0, iterations, landmarks, [0, len(landmarks)], True, ctx)[0][0]
 
 
-def observation_losses(poses, bearings, offsets, ctx=None):
-    """observation_loss of every observation of L landmarks (observation lists as in LinearEigenTriangulator.triangulate_batch)"""
+def observation_losses(poses, bearings, offsets, ctx=None, triangulator=None):
+    """observation_loss of every observation of L landmarks (observation lists as in LinearEigenTriangulator.triangulate_batch).
+    triangulator: VSlam's triangulator for the landmarks of three or more observations (a LinearEigen, SineL1 or MeanMean
+    Triangulator from cv_b200.triangulation); None is LinearEigenTriangulator's default."""
     ctx, L = _lib(ctx)
     p = _poses_in(poses); b = _f64(bearings, 3)
     off = np.ascontiguousarray(offsets, np.uint32)
     out = np.zeros(len(b), np.float64)
-    ctx.check(L.cvb_observation_losses(ctx.handle, p.ctypes.data, b.ctypes.data, off.ctypes.data, len(off) - 1, out.ctypes.data))
+    if triangulator is None:
+        ctx.check(L.cvb_observation_losses(ctx.handle, p.ctypes.data, b.ctypes.data, off.ctypes.data, len(off) - 1, out.ctypes.data))
+    else:
+        ctx, L = _tri_lib(ctx)
+        ctx.check(L.cvb_observation_losses_tri(ctx.handle, C.byref(triangulator.cfg), p.ctypes.data, b.ctypes.data, off.ctypes.data,
+                                               len(off) - 1, out.ctypes.data))
     return out
 
 
-def tri_landmarks_robust(first_pose, second_pose, observations, maximum_cosine_distance, incidence_minimum_cosine_distance, ctx=None):
-    """is_tri_landmark_robust for n (centre, first, second) bearing triples of one view triple -> bool[n]"""
+def tri_landmarks_robust(first_pose, second_pose, observations, maximum_cosine_distance, incidence_minimum_cosine_distance, ctx=None,
+                         triangulator=None):
+    """is_tri_landmark_robust for n (centre, first, second) bearing triples of one view triple -> bool[n].  triangulator: as in
+    observation_losses."""
     ctx, L = _lib(ctx)
     p = _poses_in([first_pose, second_pose])
     o = np.ascontiguousarray(observations, np.float64).reshape(-1, 9)
     out = np.zeros(len(o), np.uint8)
-    ctx.check(L.cvb_tri_landmarks_robust(ctx.handle, p[0:1].ctypes.data, p[1:2].ctypes.data, o.ctypes.data, len(o), maximum_cosine_distance,
-                                         incidence_minimum_cosine_distance, out.ctypes.data))
+    if triangulator is None:
+        ctx.check(L.cvb_tri_landmarks_robust(ctx.handle, p[0:1].ctypes.data, p[1:2].ctypes.data, o.ctypes.data, len(o), maximum_cosine_distance,
+                                             incidence_minimum_cosine_distance, out.ctypes.data))
+    else:
+        ctx, L = _tri_lib(ctx)
+        ctx.check(L.cvb_tri_landmarks_robust_tri(ctx.handle, C.byref(triangulator.cfg), p[0:1].ctypes.data, p[1:2].ctypes.data, o.ctypes.data,
+                                                 len(o), maximum_cosine_distance, incidence_minimum_cosine_distance, out.ctypes.data))
     return out.astype(bool)
