@@ -12,7 +12,8 @@
 //   k_ars_estimate  eight-point / P3P / five-point per hypothesis (k_estimate's device functions); k_ars_estimate8<L>: eight-point
 //                   with L lanes per hypothesis on the round-robin Jacobi (geom.cu: sym_eigen9_rr)
 //   k_ars_score     one warp per (model, 32 data): inlier bits by ballot.  CameraToCamera bits come from the exact-predicate
-//                   filter (c2c_filter.cuh) with the Jacobi evaluation as fallback
+//                   filter (c2c_filter.cuh); the predicates it leaves undecided are queued for the Jacobi evaluation
+//   k_ars_resolve   the queued predicates, one per thread (k_ars_resolve_block: those of a block iteration's scoring)
 //   k_ars_sprt      one CTA: the adaptive SPRT over all initial models in order.  Up to 1024 models are walked concurrently under
 //                   the state in front of the chunk; a walk carries the exact likelihood ratio and both corners of nested BOXES of
 //                   delta values -- f32 multiplication is monotone, so a model whose corners stop where the exact walk stops has
@@ -30,7 +31,7 @@
 #define ARS_SORT_CAP 4096u     // max_candidate_hypotheses + estimations_per_block * models_per_sample must fit
 #define ARS_BOOK_NT 1024
 #define ARS_BOOK_SMEM (14u * ARS_SORT_CAP)
-#define ARS_QCAP (1u << 20)    // queue of undecided predicates of the initial scoring (entries beyond it are evaluated in place)
+#define ARS_QCAP (1u << 20)    // queue of undecided predicates of a scoring stage (entries beyond it are evaluated in place)
 
 struct ArrsacCtl {
     uint32_t n, init_n, Mv, npass;
@@ -47,6 +48,7 @@ struct ArrsacCtl {
     uint32_t stat_chunks, stat_pass;
     uint32_t stat_walk_us, stat_commit_us;   // SPRT: time in the chunk walks / in the commit turns (globaltimer)
     uint32_t stat_perm_us, stat_turns;       // SPRT: time in the ordering step in front of the walks; commit turns in total
+    uint32_t q_blk, stat_qblk;               // undecided predicates queued by the current block's scoring (queue region 0); over all blocks
 };
 
 struct ArrsacParams {            // launch-constant configuration (by value)
@@ -231,6 +233,7 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_begin(ArrsacCtl *ctl, Arrsa
         ctl->Mv = 0; ctl->npass = 0; ctl->Hn = 0; ctl->cur = 0; ctl->blk_lo = ctl->blk_hi = ctl->acc_hi = 0;
         ctl->n_new = 0; ctl->worst = 0; ctl->found = 0; ctl->iters = 0; ctl->n_inliers = 0; ctl->overflow = 0;
         ctl->stat_chunks = 0; ctl->stat_pass = 0; ctl->q_count = 0; ctl->q_count2 = 0; ctl->stat_lazy = 0; ctl->stat_units0 = 0; ctl->stat_units2 = 0; ctl->stat_repairs = 0; ctl->stat_pad = 0; ctl->stat_walk_us = 0; ctl->stat_commit_us = 0; ctl->stat_perm_us = 0; ctl->stat_turns = 0;
+        ctl->q_blk = 0; ctl->stat_qblk = 0;
         ctl->done = (n < P.K || P.H0 == 0) ? 1u : 0u;
     }
     __syncthreads();
@@ -294,6 +297,21 @@ __device__ __forceinline__ bool ars_inlier(const cvb_pose &Pz, const double *__r
     return f != 0;
 }
 
+// the scoring kernels' predicate: the exact evaluation costs ~8x the filter, so an undecided pair goes to a queue that a resolve
+// kernel works off without divergence (one undecided lane would otherwise stall its warp for the whole Jacobi iteration) and
+// counts as an outlier until then; `src` tells the resolve kernel which pose and mask row the entry belongs to
+template <int RES>
+__device__ __forceinline__ bool ars_inlier_queued(const cvb_pose &Pz, const double *__restrict__ a, const double *__restrict__ b, uint32_t i,
+                                                  double thr, uint32_t *qc, uint2 *q, uint32_t src) {
+    if (RES == 1) return ars_inlier<RES>(Pz, a, b, i, thr);
+    const double *pa = a + 3 * (size_t)i, *pb = b + 3 * (size_t)i;
+    const int f = c2c_inlier_filter(Pz.r, Pz.t, pa, pb, thr);
+    if (f >= 0) return f != 0;
+    const uint32_t slot = atomicAdd(qc, 1u);
+    if (slot < ARS_QCAP) { q[slot] = make_uint2(src, i); return false; }
+    return ars_exact_c2c(&Pz, pa, pb, thr);
+}
+
 // are the mask words >= 1 of an initial model computed by the scoring kernels?  (word0 = its final first mask word)
 __device__ __forceinline__ bool ars_ready(uint32_t word0, uint32_t init_n, uint32_t sample, const ArrsacParams &P) {
     if (sample < P.prefix) return true;
@@ -332,21 +350,7 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
             if (phase == 2 && !ars_ready(masks0[(size_t)m * P.W0], init_n, m / P.MM, P)) continue;
             const uint32_t i = w * 32 + lane;
             bool bit = false;
-            if (i < init_n) {
-                if (RES == 1) bit = ars_inlier<RES>(poses0[m], a, b, i, P.thr);
-                else {
-                    // the exact evaluation costs ~8x the filter: undecided pairs go to a queue that k_ars_resolve works off
-                    // without divergence (one undecided lane would otherwise stall its warp for the whole Jacobi iteration)
-                    const cvb_pose &Pz = poses0[m];
-                    const int f = c2c_inlier_filter(Pz.r, Pz.t, a + 3 * (size_t)i, b + 3 * (size_t)i, P.thr);
-                    if (f >= 0) bit = f != 0;
-                    else {
-                        const uint32_t slot = atomicAdd(qc, 1u);
-                        if (slot < ARS_QCAP) q[slot] = make_uint2(m, i);
-                        else bit = ars_exact_c2c(&Pz, a + 3 * (size_t)i, b + 3 * (size_t)i, P.thr);
-                    }
-                }
-            }
+            if (i < init_n) bit = ars_inlier_queued<RES>(poses0[m], a, b, i, P.thr, qc, q, m);      // queue: k_ars_resolve
             const unsigned bits = __ballot_sync(full, bit);
             if (lane == 0) { masks0[(size_t)m * P.W0 + w] = bits; atomicAdd(phase == 0 ? &ctl->stat_units0 : &ctl->stat_units2, 1u); }
         }
@@ -359,13 +363,15 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
     const uint32_t units = kept_units + nnew * nwn;
     const cvb_pose *tp = tposes + (size_t)cur * P.rows;
     uint32_t *tm = tmasks + (size_t)cur * P.rows * P.NW;
+    // undecided predicates go to queue region 0 (free once the initial stages are resolved) for k_ars_resolve_block:
+    // entry source r < P.rows is kept row r, P.rows + j is new model j
     for (uint32_t u = warp; u < units; u += nwarps) {
         if (u < kept_units) {
             const uint32_t r = u / nwb, w = wlo + u % nwb;
             const uint32_t i = w * 32 + lane;
             const bool act = i >= lo && i < hi;
             bool bit = false;
-            if (act) bit = ars_inlier<RES>(tp[r], a, b, i, P.thr);
+            if (act) bit = ars_inlier_queued<RES>(tp[r], a, b, i, P.thr, &ctl->q_blk, queue, r);
             const unsigned bits = __ballot_sync(full, bit), range = __ballot_sync(full, act);
             if (lane == 0) { uint32_t *p = tm + (size_t)r * P.NW + w; *p = (*p & ~range) | bits; }
         } else {
@@ -374,7 +380,7 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
             if ((j % P.MM) >= nposes_new[j / P.MM]) continue;
             const uint32_t i = w * 32 + lane;
             bool bit = false;
-            if (i < hi) bit = ars_inlier<RES>(newposes[j], a, b, i, P.thr);
+            if (i < hi) bit = ars_inlier_queued<RES>(newposes[j], a, b, i, P.thr, &ctl->q_blk, queue, P.rows + j);
             const unsigned bits = __ballot_sync(full, bit);
             if (lane == 0) newmask[(size_t)j * P.NW + w] = bits;
         }
@@ -392,6 +398,23 @@ __global__ void __launch_bounds__(256) k_ars_resolve(const ArrsacCtl *ctl, const
         const uint2 q = queue[e];
         if (residual_c2c(poses0[q.x], a + 3 * (size_t)q.y, b + 3 * (size_t)q.y) < P.thr)
             atomicOr(&masks0[(size_t)q.x * P.W0 + (q.y >> 5)], 1u << (q.y & 31));
+    }
+}
+
+// the same for the block loop's scoring (k_ars_score phase 1, in front of k_ars_book): inliers are OR-ed into the mask rows of the
+// current candidate table and into newmask
+__global__ void __launch_bounds__(64) k_ars_resolve_block(const ArrsacCtl *ctl, const uint2 *__restrict__ queue, ArrsacParams P,
+                                                          const double *__restrict__ a, const double *__restrict__ b,
+                                                          const cvb_pose *__restrict__ tposes, uint32_t *__restrict__ tmasks,
+                                                          const cvb_pose *__restrict__ newposes, uint32_t *__restrict__ newmask) {
+    if (ctl->done) return;
+    const uint32_t cnt = min(ctl->q_blk, ARS_QCAP), cur = ctl->cur;
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < cnt; e += gridDim.x * blockDim.x) {
+        const uint2 q = queue[e];
+        const bool kept = q.x < P.rows;
+        const size_t row = kept ? (size_t)cur * P.rows + q.x : (size_t)(q.x - P.rows);
+        if (residual_c2c(kept ? tposes[row] : newposes[row], a + 3 * (size_t)q.y, b + 3 * (size_t)q.y) < P.thr)
+            atomicOr(&(kept ? tmasks : newmask)[row * P.NW + (q.y >> 5)], 1u << (q.y & 31));
     }
 }
 
@@ -864,6 +887,7 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_book(ArrsacCtl *ctl, Arrsac
     uint32_t *e_inl = (uint32_t *)(ars_dyn + 8 * ARS_SORT_CAP);                  // inliers by entry position (part 1 order)
     uint16_t *e_src = (uint16_t *)(ars_dyn + 12 * ARS_SORT_CAP);                 // source: < rows -> kept row of the current table, else rows + new model
     const uint32_t tid = threadIdx.x, NT = blockDim.x;
+    if (tid == 0) { ctl->stat_qblk += ctl->q_blk; ctl->q_blk = 0; }      // this block's queue has been resolved
     const uint32_t cur = ctl->cur, Hk = ctl->Hn, n = ctl->n;
     const uint32_t acc_hi = ctl->acc_hi, lo = ctl->blk_lo, hi = ctl->blk_hi, worst = ctl->worst;
     const uint32_t nnew = ctl->n_new * P.MM;

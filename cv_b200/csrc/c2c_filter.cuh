@@ -15,10 +15,13 @@
 //       (Sylvester's law of inertia).  Exactly one negative pivot at s_lo and exactly one at s_hi = min(1024 s_lo, 0.01)
 //       (>= 16 s_lo, else the filter declines) gives l1 < s_lo < s_hi < l2: inverse iteration with shift s_lo then contracts
 //       the error by <= s_lo / (s_hi - s_lo) <= 1/15 per step (1e-3 at the production threshold 1e-7), and a final step that
-//       turns the vector by < 1e-11 certifies the eigenvector to ~1e-12.
+//       turns the vector by < 1e-11 certifies the eigenvector to ~1e-12 (error after the step <= turn * c / (1 - c) at contraction c).
+//       When the count at s_hi is not 1 (small gap l2: low parallax), lower upper shifts s_hi / 8, s_hi / 64, ... down to 16 s_lo
+//       are tried: exactly one negative pivot at any of them gives l1 < s_lo < s < l2 and a contraction <= 1/15, which is the case the
+//       certificate above is sized for, so the same turn tolerance and residual band apply; only more checked steps may be needed.
 //   (3) the residual of that eigenvector is computed with the reference's formula; if it is further from the threshold
 //       than 1e-11 + 1e-4 thr (orders of magnitude above the rounding of either evaluation) the comparison is decided.
-//   Anything else (tiny pivots, l2 < s_hi, non-finite values, slow convergence, residual inside the band, thresholds so
+//   Anything else (tiny pivots, l2 < 16 s_lo, non-finite values, slow convergence, residual inside the band, thresholds so
 //   large that s_hi is not small) returns -1.
 //
 // Compiles for the device (nvcc) and for the host (g++; only the CPU tests do that, to compare every decision with the exact CPU evaluation).
@@ -153,7 +156,12 @@ C2C_HD int c2c_inlier_filter(const double *R, const double *t, const double *a, 
     const int c_lo = c2c_ldl4(D, s_lo, d, l, id);
     if (c_lo == 0) return 0;                       // l1 > s_lo: residual >= 2 thr
     if (c_lo != 1) return -1;
-    if (c2c_ldl4(D, s_hi, dh, lh, ih) != 1) return -1; // need l2 > s_hi for the contraction bound
+    // need l2 > s for the contraction bound: s = s_hi, then a ladder of lower shifts down to 16 s_lo (small spectral gap, low
+    // parallax).  Every rung keeps the contraction <= s_lo / (s - s_lo) <= 1/15, the worst case the certificate below is sized for.
+    for (double s = s_hi; c2c_ldl4(D, s, dh, lh, ih) != 1;) {
+        s *= 0.125;
+        if (!(s >= 16.0 * s_lo)) return -1;
+    }
     id[3] = 1.0 / d[3];
     // inverse iteration with shift s_lo.  Four solves without normalisation (growth <= 1 / |l1 - s_lo| per solve, harmless in
     // f64; error <= 1e-12 at the production threshold), one normalisation, then a checked step y = (D - s_lo I)^-1 x: the
@@ -169,7 +177,7 @@ C2C_HD int c2c_inlier_filter(const double *R, const double *t, const double *a, 
     c2c_normalise4(x);
     double y[4], yy = 0.0;
     int certified = 0;
-    for (int it = 0; it < 4; it++) {
+    for (int it = 0; it < 12; it++) {            // at contraction 1/15: 4 blind + 12 checked steps take an error of 10^7 below 1e-11
         y[0] = x[0]; y[1] = x[1]; y[2] = x[2]; y[3] = x[3];
         c2c_ldl4_solve(id, l, y);
         const double xy = c2c_dot4(x, y);

@@ -1408,12 +1408,12 @@ struct ArsWorkspace {
         ArrsacParams P; int kind, row0; const void *a, *b, *n_dev; uint32_t n_host, nmax, cap, nb; const void *model, *inl, *ninl, *found;
         const void *ws[21];
     };
-    struct GraphEntry { GraphKey key; cudaGraphExec_t exec; uint64_t launches; bool loop; };
-    bool last_loop = false;         // the pending run went through a WHILE-node graph (its body's launches are counted at commit)
+    struct GraphEntry { GraphKey key; cudaGraphExec_t exec; uint64_t launches; uint32_t body; };   // body: launches of one WHILE body (0: no WHILE node)
+    uint32_t last_body = 0;         // the pending run went through a WHILE-node graph with this many launches per body (counted at commit)
     std::vector<GraphEntry> graphs;
     std::vector<GraphKey> seen;
     int use_graph = -1;             // CVB_NO_GRAPH=1 / CVB_ARS_NO_GRAPH=1 disable
-    // the block loop as a WHILE node of the graph (body: score, book, estimate; k_ars_book clears the condition at the loop's
+    // the block loop as a WHILE node of the graph (body: score, resolve, book, estimate; k_ars_book clears the condition at the loop's
     // end) instead of one unrolled body per possible data block.  CVB_ARS_WHILE=0 keeps the unrolled graph.
     int use_while = -1;
     cudaStream_t body_stream = nullptr;
@@ -1759,6 +1759,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         attr_set = true;
     }
     bool capturing = false, while_loop = false;
+    uint32_t body_launches = 0;
     // everything the stream sees, from the upload of the draw stream to the copy of the control block back
     auto enqueue = [&]() -> int {
         CVB_CUDA(ctx, cudaMemcpyAsync(w->ctl.p, w->h_raw, sizeof(ArrsacCtl), cudaMemcpyHostToDevice, st));
@@ -1849,6 +1850,18 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
+        // a block's score, the exact evaluation of the predicates it queued (CameraToCamera only), its bookkeeping
+        auto score_block = [&](unsigned long long cond) -> int {
+            if ((rc = score(1))) return rc;
+            if (res == 0) {
+                CVB_PROF(ctx, "k_ars_resolve_block", 0);
+                // 64-thread CTAs: a block queues a small fraction of its predicates, spread over as many SMs as possible
+                k_ars_resolve_block<<<sgrid_full, 64, 0, st>>>(ctl, (const uint2 *)w->queue.p, P, a_dev, b_dev, (const cvb_pose *)w->tposes.p,
+                                                               (uint32_t *)w->tmasks.p, (const cvb_pose *)w->newposes.p, (uint32_t *)w->newmask.p);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            return book(cond);
+        };
         if (capturing && while_loop) {
             // device-side loop: one WHILE node whose body is one block iteration; k_ars_book ends it (block nb at the latest: lo >= n)
             cudaStreamCaptureStatus cs;
@@ -1868,9 +1881,10 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             const cudaStream_t outer = st;
             CVB_CUDA(ctx, cudaStreamBeginCaptureToGraph(w->body_stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
             st = w->body_stream;                     // the launch helpers below capture into the body (restored before any return)
-            rc = score(1);
-            if (!rc) rc = book(cond);
+            const uint64_t b0 = ctx->launches;
+            rc = score_block(cond);
             if (!rc && nb && P.G) rc = estimate(1, P.G, (const uint32_t *)w->samples_new.p, (cvb_pose *)w->newposes.p, (uint8_t *)w->nposes_new.p);
+            body_launches = (uint32_t)(ctx->launches - b0);
             cudaGraph_t same_body = nullptr;
             const cudaError_t be = cudaStreamEndCapture(st, &same_body);
             st = outer;
@@ -1879,8 +1893,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_CUDA(ctx, cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
         } else
         for (uint32_t it = 0; it <= nb; it++) {
-            if ((rc = score(1))) return rc;
-            if ((rc = book(0))) return rc;
+            if ((rc = score_block(0))) return rc;
             if (it < nb && P.G)
                 if ((rc = estimate(1, P.G, (const uint32_t *)w->samples_new.p, (cvb_pose *)w->newposes.p, (uint8_t *)w->nposes_new.p))) return rc;
         }
@@ -1919,7 +1932,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_CUDA(ctx, cudaGraphLaunch(ge.exec, st));
             CVB_CUDA(ctx, cudaEventRecord(w->up_done, st));       // replay: the staging buffer is free when the run is over
             ctx->launches += ge.launches;
-            w->last_loop = ge.loop;
+            w->last_body = ge.body;
             w->pending = true;
             return 0;
         }
@@ -1969,8 +1982,8 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         return 0;
     }
     if (w->graphs.size() >= 16) { cudaGraphExecDestroy(w->graphs.front().exec); w->graphs.erase(w->graphs.begin()); }
-    w->graphs.push_back({key, exec, ctx->launches - l0, while_loop});
-    w->last_loop = while_loop;
+    w->graphs.push_back({key, exec, ctx->launches - l0, while_loop ? body_launches : 0u});
+    w->last_body = while_loop ? body_launches : 0u;
     CVB_CUDA(ctx, cudaGraphLaunch(exec, st));
     CVB_CUDA(ctx, cudaEventRecord(w->up_done, st));
     w->pending = true;
@@ -1984,8 +1997,12 @@ int arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, ArrsacCtl *stats_out = nullptr
     if (!w->pending) return cvb_set_error(ctx, CVB_EINVAL, "no device ARRSAC run to commit");
     const ArrsacCtl *h = (const ArrsacCtl *)w->h_res;
     if (stats_out) *stats_out = *h;
-    if (w->last_loop) ctx->launches += 3ull * h->iters;           // the WHILE body ran iters + 1 times, the capture counted it once
-    w->last_loop = false;
+    if (getenv("CVB_ARS_DEBUG"))
+        fprintf(stderr, "[arrsac] n %u models %u pass %u chunks %u turns %u repairs %u lazy %u | sprt us: order %u walk %u commit %u | block iterations %u"
+                " | undecided predicates queued: initial %u block %u\n", h->n, h->Mv, h->npass, h->stat_chunks, h->stat_turns, h->stat_repairs,
+                h->stat_lazy, h->stat_perm_us, h->stat_walk_us, h->stat_commit_us, h->iters, h->q_count + h->q_count2, h->stat_qblk);
+    ctx->launches += (uint64_t)w->last_body * h->iters;          // the WHILE body ran iters + 1 times, the capture counted it once
+    w->last_body = 0;
     w->pending = false;
     if (!rng) return 0;
     const uint64_t used = h->rng_pos;
@@ -2344,9 +2361,6 @@ int cvb_arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, uint32_t *stats_out) {
     ArrsacCtl h;
     int rc = arrsac_commit_rng(ctx, rng, &h);
     if (rc) return rc;
-    if (getenv("CVB_ARS_DEBUG"))
-        fprintf(stderr, "[arrsac] n %u models %u pass %u chunks %u turns %u repairs %u lazy %u | sprt us: order %u walk %u commit %u | block iterations %u\n", h.n, h.Mv, h.npass,
-                h.stat_chunks, h.stat_turns, h.stat_repairs, h.stat_lazy, h.stat_perm_us, h.stat_walk_us, h.stat_commit_us, h.iters);
     if (stats_out) {   // 16 words (13..15 reserved): n, valid initial models, SPRT passes, SPRT commit rounds, block iterations, draws, inliers, found, 32-datum units
                        // scored in stage 1 / stage 2, predicates resolved exactly from the queues, mask words computed by the SPRT itself, SPRT repairs
         stats_out[0] = h.n; stats_out[1] = h.Mv; stats_out[2] = h.npass; stats_out[3] = h.stat_chunks; stats_out[4] = h.iters;
