@@ -183,3 +183,6 @@ pub use sfm::*;
 // ---- INTEGRATION.md section 2d (include/cvb200_tri.h) ----
 mod tri;
 pub use tri::*;
+
+// ---- INTEGRATION.md section 2e (include/cvb200_opt.h) ----
+pub mod opt;

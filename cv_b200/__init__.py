@@ -9,6 +9,7 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   CameraIntrinsics(K1Distortion) <- cv-pinhole/src/lib.rs:32-240
   frame_features        <- cv-sfm VSlam::kps_descriptors        (cv-sfm/src/lib.rs:2195-2235)
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
+  *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
 There is no CPU fallback: every call runs CUDA kernels from cv_b200/libcvb200.so and raises
 CvbError when the library or a Hopper (sm_90) GPU is missing.
@@ -21,9 +22,10 @@ from .geom import (Arrsac, EightPoint, LambdaTwist, NisterStewenius, Pcg64, Xosh
                    residuals_camera_to_camera, residuals_world_to_camera)
 from .triangulation import (AngularL1Triangulator, AngularLInfinityTriangulator, LinearEigenTriangulator,  # noqa: F401
                             MeanMeanTriangulator, RelativeDltTriangulator, SineL1Triangulator)
-from .optimize import (observation_losses, single_view_simple_optimize_l2, single_view_simple_optimize_l2_batch,  # noqa: F401
-                       three_view_adaptive_optimize_l2, three_view_optimize_l2_batch, three_view_simple_optimize_l2,
-                       tri_landmarks_robust)
+from .optimize import (observation_losses, single_view_simple_optimize_l1, single_view_simple_optimize_l1_batch,  # noqa: F401
+                       single_view_simple_optimize_l2, single_view_simple_optimize_l2_batch, three_view_adaptive_optimize_l2,
+                       three_view_optimize_l2_batch, three_view_simple_optimize_l1, three_view_simple_optimize_l1_batch,
+                       three_view_simple_optimize_l2, tri_landmarks_robust)
 from .sfm_match import landmark_matches  # noqa: F401
 from . import checkpoint  # noqa: F401  (bincode record images of the VSlamData checkpoint)
 from .pair import Intrinsics, IntrinsicsK1, TwoViewBuffers, two_view_frames  # noqa: F401

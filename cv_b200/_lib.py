@@ -1,4 +1,5 @@
-"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h)."""
+"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its module
+cv_b200/libcvb200_opt.so (include/cvb200_opt.h)."""
 import ctypes as C
 import os
 
@@ -65,6 +66,11 @@ TRI_ABI_SYMBOLS = [
     "cvb_tri_landmarks_robust_tri",
 ]
 
+# every symbol include/cvb200_opt.h declares (cv-optimize's L1 optimizers), exported by libcvb200_opt.so; checked by tests/test_abi_opt.py
+OPT_ABI_SYMBOLS = [
+    "cvb_single_view_optimize_l1", "cvb_three_view_optimize_l1",
+]
+
 
 def lib_path():
     return os.path.join(_HERE, "libcvb200.so")
@@ -117,6 +123,25 @@ def load_library():
     L.cvb_hash_bag_dev.argtypes = [vp, vp, vp, u32, vp, u32, vp]
     _LIB = L
     return L
+
+
+_OPT_LIB = None
+
+
+def opt_lib_path():
+    return os.path.join(_HERE, "libcvb200_opt.so")
+
+
+def load_opt_library():
+    """Loads libcvb200_opt.so, the module of include/cvb200_opt.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _OPT_LIB
+    if _OPT_LIB is None:
+        load_library()
+        p = opt_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        _OPT_LIB = C.CDLL(p)
+    return _OPT_LIB
 
 
 class Context:

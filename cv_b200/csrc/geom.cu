@@ -14,6 +14,7 @@
 #include <vector>
 #include "common.cuh"
 #include "../../include/cvb200_tri.h"
+#include "../../include/cvb200_opt.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1100,6 +1101,122 @@ __global__ void __launch_bounds__(OPT_NT) k_three_view_opt(const cvb_pose *__res
                     }
                 }
                 if (stop) s_stop = 1;
+                else {
+                    apply_delta(d, d + 3, &P[0]); apply_delta(d + 6, d + 9, &P[1]); updates++;
+                    if (it == iterations - 1) s_stop = 1;
+                }
+            }
+            __syncthreads();
+            if (s_stop) break;
+        }
+    if (threadIdx.x == 0) {
+        if (n > 0) { pose_inverse(P[0], &poses_out[2 * b]); pose_inverse(P[1], &poses_out[2 * b + 1]); }
+        else { poses_out[2 * b] = poses_in[2 * b]; poses_out[2 * b + 1] = poses_in[2 * b + 1]; }
+        updates_out[b] = updates;
+    }
+}
+
+// cv-optimize's L1 (Weiszfeld) optimizers (include/cvb200_opt.h): the L2 kernels' shape, with per pose the sums of
+// g.l1() = Se3TangentSpace::new(t.normalize(), r.normalize()) (so3.rs:23-34,123-125; a zero gradient normalises to NaN and
+// becomes zero, but its weights still count) and of the weights 1/(|g.t| + tscale ε), 1/(|g.r| + ε).
+// l1 += g.l1(), w[0] += translation weight, w[1] += rotation weight (single_view_optimizer.rs:36-38, three_view_optimizer.rs:53-55)
+__device__ __forceinline__ void l1_accumulate(const double *tg, const double *rg, double tse, double eps, double *l1, double *w) {
+    double lt[3], lr[3];
+    w[0] += 1.0 / (norm3(tg) + tse);
+    w[1] += 1.0 / (norm3(rg) + eps);
+    normalize3(tg, lt); normalize3(rg, lr);
+    tangent_new(lt, lr);
+    for (int k = 0; k < 3; k++) { l1[k] += lt[k]; l1[3 + k] += lr[k]; }
+}
+// l1sum.scale(rate).scale_translation(ts.recip()).scale_rotation(rs.recip()): multiply by rate first, then by the reciprocal
+__device__ __forceinline__ void l1_delta(const double *l1, const double *w, double rate, double *d) {
+    const double it = 1.0 / w[0], ir = 1.0 / w[1];
+    for (int k = 0; k < 3; k++) { d[k] = (l1[k] * rate) * it; d[3 + k] = (l1[3 + k] * rate) * ir; }
+}
+
+// single_view_optimizer.rs:16-78, one CTA per (pose, landmark list); acc = [l1sum.t, l1sum.r, ts, rs]
+__global__ void __launch_bounds__(OPT_NT) k_single_view_opt_l1(const cvb_pose *__restrict__ poses_in, const double *__restrict__ bearings,
+                                                               const double *__restrict__ world, const uint32_t *__restrict__ offsets,
+                                                               double eps, double rate, uint32_t iterations, cvb_pose *__restrict__ poses_out,
+                                                               uint32_t *__restrict__ updates_out) {
+    __shared__ cvb_pose P;
+    __shared__ double s_red[OPT_WARPS * 8];
+    __shared__ int s_stop;
+    const uint32_t b = blockIdx.x, o0 = offsets[b], n = offsets[b + 1] - o0;
+    if (threadIdx.x == 0) { P = poses_in[b]; s_stop = 0; }
+    __syncthreads();
+    double best_t = INFINITY, best_r = INFINITY;
+    uint32_t no_improve = 0, updates = 0;
+    if (n > 0)
+        for (uint32_t it = 0; it < iterations; it++) {
+            double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tg[3], rg[3];
+            const cvb_pose Pl = P;
+            const double tse = norm3(Pl.t) * eps;       // tscale of the current pose (:30)
+            for (uint32_t i = threadIdx.x; i < n; i += OPT_NT)
+                if (landmark_delta(Pl, bearings + 3 * (size_t)(o0 + i), world + 4 * (size_t)(o0 + i), tg, rg))
+                    l1_accumulate(tg, rg, tse, eps, acc, acc + 6);
+            block_sum<8>(acc, s_red);
+            if (threadIdx.x == 0) {
+                double d[6];
+                l1_delta(acc, acc + 6, rate, d);
+                no_improve++;
+                const double t = norm3(acc), r = norm3(acc + 3);   // patience on the unnormalised l1sum (:47-57)
+                if (best_t > t) { best_t = t; no_improve = 0; }
+                if (best_r > r) { best_r = r; no_improve = 0; }
+                if (no_improve >= 50) s_stop = 1;
+                else {
+                    apply_delta(d, d + 3, &P); updates++;
+                    if (it == iterations - 1) s_stop = 1;
+                }
+            }
+            __syncthreads();
+            if (s_stop) break;
+        }
+    if (threadIdx.x == 0) { poses_out[b] = P; updates_out[b] = updates; }
+}
+
+// three_view_optimizer.rs:23-124, one CTA per (pose pair, observation triples); acc = [l1sum0 (6), l1sum1 (6), ts0, rs0, ts1, rs1]
+__global__ void __launch_bounds__(OPT_NT) k_three_view_opt_l1(const cvb_pose *__restrict__ poses_in, const double *__restrict__ obs,
+                                                              const uint32_t *__restrict__ offsets, double eps, double rate,
+                                                              uint32_t iterations, cvb_pose *__restrict__ poses_out,
+                                                              uint32_t *__restrict__ updates_out) {
+    __shared__ cvb_pose P[2];
+    __shared__ double s_red[OPT_WARPS * 16];
+    __shared__ int s_stop;
+    const uint32_t b = blockIdx.x, o0 = offsets[b], n = offsets[b + 1] - o0;
+    if (threadIdx.x == 0) {
+        if (n > 0) { pose_inverse(poses_in[2 * b], &P[0]); pose_inverse(poses_in[2 * b + 1], &P[1]); }
+        s_stop = 0;
+    }
+    __syncthreads();
+    double best[2][2] = {{INFINITY, INFINITY}, {INFINITY, INFINITY}};
+    uint32_t no_improve = 0, updates = 0;
+    if (n > 0)
+        for (uint32_t it = 0; it < iterations; it++) {
+            double acc[16], g[12];
+            for (int k = 0; k < 16; k++) acc[k] = 0.0;
+            const cvb_pose P0 = P[0], P1 = P[1];
+            const double tse = (norm3(P0.t) + norm3(P1.t)) * eps;   // tscale of the inverted poses (:45-48)
+            for (uint32_t i = threadIdx.x; i < n; i += OPT_NT) {
+                const double *o = obs + 9 * (size_t)(o0 + i);
+                double f[3], s[3];
+                rotv(P0.r, o + 3, f); rotv(P1.r, o + 6, s);
+                three_view_gradients(o, f, P0.t, s, P1.t, g);
+                l1_accumulate(g, g + 3, tse, eps, acc, acc + 12);
+                l1_accumulate(g + 6, g + 9, tse, eps, acc + 6, acc + 14);
+            }
+            block_sum<16>(acc, s_red);
+            if (threadIdx.x == 0) {
+                double d[12];
+                l1_delta(acc, acc + 12, rate, d);
+                l1_delta(acc + 6, acc + 14, rate, d + 6);
+                no_improve++;
+                for (int v = 0; v < 2; v++) {          // one patience counter over all four norms (:69-81)
+                    const double t = norm3(acc + 6 * v), r = norm3(acc + 6 * v + 3);
+                    if (best[v][0] > t) { best[v][0] = t; no_improve = 0; }
+                    if (best[v][1] > r) { best[v][1] = r; no_improve = 0; }
+                }
+                if (no_improve >= 50) s_stop = 1;
                 else {
                     apply_delta(d, d + 3, &P[0]); apply_delta(d + 6, d + 9, &P[1]); updates++;
                     if (it == iterations - 1) s_stop = 1;
@@ -2426,6 +2543,67 @@ int cvb_three_view_optimize_l2(cvb_ctx *ctx, const cvb_pose *poses, uint32_t B, 
     }
     return download_poses_updates(ctx, g, poses_out, 2 * (size_t)B, updates_out, B);
 }
+
+}  // extern "C"
+
+// The entry points of include/cvb200_opt.h are exported by libcvb200_opt.so (cv_b200/csrc/opt.cu), a module over this library, so
+// that libcvb200.so keeps exporting exactly the C ABI of cvb200.h, cvb200_sfm.h and cvb200_tri.h.  These are their implementations,
+// with C++ linkage like the other functions shared between this library's translation units.
+int opt_single_view_l1(cvb_ctx *ctx, const cvb_pose *poses, uint32_t B, double epsilon, double optimization_rate, uint32_t iterations,
+                        const double *bearings, const double *world, const uint32_t *offsets,
+                                cvb_pose *poses_out, uint32_t *updates_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (B == 0) return 0;
+    if (!poses || !offsets || !poses_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    int rc;
+    if ((rc = offsets_check(ctx, offsets, B))) return rc;
+    const uint32_t n = offsets[B];
+    if (n && (!bearings || !world)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * (size_t)B))) return rc;
+    if ((rc = upload(ctx, g->a, bearings, sizeof(double) * 3 * (size_t)n))) return rc;
+    if ((rc = upload(ctx, g->b, world, sizeof(double) * 4 * (size_t)n))) return rc;
+    if ((rc = upload(ctx, g->offsets, offsets, sizeof(uint32_t) * ((size_t)B + 1)))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(cvb_pose) * (size_t)B))) return rc;
+    if ((rc = g->ok.ensure(ctx, sizeof(uint32_t) * (size_t)B))) return rc;
+    {
+        CVB_PROF(ctx, "k_single_view_opt_l1", 0.0);
+        k_single_view_opt_l1<<<B, OPT_NT, 0, ctx->stream>>>((const cvb_pose *)g->poses.p, (const double *)g->a.p, (const double *)g->b.p,
+                                                            (const uint32_t *)g->offsets.p, epsilon, optimization_rate, iterations,
+                                                            (cvb_pose *)g->out.p, (uint32_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return download_poses_updates(ctx, g, poses_out, (size_t)B, updates_out, B);
+}
+
+int opt_three_view_l1(cvb_ctx *ctx, const cvb_pose *poses, uint32_t B, double epsilon, double optimization_rate, uint32_t iterations,
+                       const double *observations, const uint32_t *offsets, cvb_pose *poses_out,
+                               uint32_t *updates_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (B == 0) return 0;
+    if (!poses || !offsets || !poses_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    int rc;
+    if ((rc = offsets_check(ctx, offsets, B))) return rc;
+    const uint32_t n = offsets[B];
+    if (n && !observations) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * 2 * (size_t)B))) return rc;
+    if ((rc = upload(ctx, g->a, observations, sizeof(double) * 9 * (size_t)n))) return rc;
+    if ((rc = upload(ctx, g->offsets, offsets, sizeof(uint32_t) * ((size_t)B + 1)))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(cvb_pose) * 2 * (size_t)B))) return rc;
+    if ((rc = g->ok.ensure(ctx, sizeof(uint32_t) * (size_t)B))) return rc;
+    {
+        CVB_PROF(ctx, "k_three_view_opt_l1", 0.0);
+        k_three_view_opt_l1<<<B, OPT_NT, 0, ctx->stream>>>((const cvb_pose *)g->poses.p, (const double *)g->a.p, (const uint32_t *)g->offsets.p,
+                                                           epsilon, optimization_rate, iterations, (cvb_pose *)g->out.p, (uint32_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return download_poses_updates(ctx, g, poses_out, 2 * (size_t)B, updates_out, B);
+}
+
+extern "C" {
 
 int cvb_observation_losses_tri(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses, const double *bearings,
                                const uint32_t *offsets, uint32_t L, double *loss_out) {

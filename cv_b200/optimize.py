@@ -1,6 +1,9 @@
-"""Host-side mirror of the steps that follow the consensus stage in cv-sfm, over the C ABI (include/cvb200.h):
+"""Host-side mirror of the steps that follow the consensus stage in cv-sfm, over the C ABI (include/cvb200.h, and
+include/cvb200_opt.h for the L1 optimizers):
 
+  single_view_simple_optimize_l1   <- cv-optimize/src/single_view_optimizer.rs:16-78
   single_view_simple_optimize_l2   <- cv-optimize/src/single_view_optimizer.rs:80-135
+  three_view_simple_optimize_l1    <- cv-optimize/src/three_view_optimizer.rs:23-124
   three_view_simple_optimize_l2    <- cv-optimize/src/three_view_optimizer.rs:126-201
   three_view_adaptive_optimize_l2  <- cv-optimize/src/three_view_optimizer.rs:203-272
   observation_losses               <- VSlam::observation_loss, cv-sfm/src/lib.rs:2570-2620
@@ -13,7 +16,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import default_context
+from ._lib import default_context, load_opt_library
 from .geom import POSE_DTYPE, _f64, _poses_in
 from .triangulation import _lib as _tri_lib
 
@@ -28,6 +31,18 @@ def _lib(ctx):
         L.cvb_observation_losses.argtypes = [vp, vp, vp, vp, u32, vp]
         L.cvb_tri_landmarks_robust.argtypes = [vp, vp, vp, vp, u32, f64, f64, vp]
         L._opt_bound = True
+    return ctx, L
+
+
+def _l1_lib(ctx):
+    """the context and libcvb200_opt.so (include/cvb200_opt.h); errors are reported through the context as for every entry point"""
+    ctx = ctx or default_context(0)
+    L = load_opt_library()
+    if not getattr(L, "_l1_bound", False):
+        vp, u32, f64 = C.c_void_p, C.c_uint32, C.c_double
+        L.cvb_single_view_optimize_l1.argtypes = [vp, vp, u32, f64, f64, u32, vp, vp, vp, vp, vp]
+        L.cvb_three_view_optimize_l1.argtypes = [vp, vp, u32, f64, f64, u32, vp, vp, vp, vp]
+        L._l1_bound = True
     return ctx, L
 
 
@@ -85,6 +100,55 @@ def three_view_adaptive_optimize_l2(poses, iterations, landmarks, ctx=None):
     if len(landmarks) == 0:
         return list(poses)
     return three_view_optimize_l2_batch([poses], 0.0, iterations, landmarks, [0, len(landmarks)], True, ctx)[0][0]
+
+
+def single_view_simple_optimize_l1_batch(poses, epsilon, optimization_rate, iterations, bearings, world, offsets, ctx=None):
+    """B problems of single_view_simple_optimize_l1: poses[b] with landmarks offsets[b]..offsets[b+1] of (bearings[n,3], world[n,4])
+    -> ([(R, t)], updates[B])"""
+    ctx, L = _l1_lib(ctx)
+    p = _poses_in(poses); b = _f64(bearings, 3); w = _f64(world, 4)
+    off = np.ascontiguousarray(offsets, np.uint32)
+    nb = len(off) - 1
+    if nb != len(p) or off[-1] != len(b) or len(b) != len(w):
+        raise ValueError("offsets / poses / landmark arrays disagree")
+    out = np.zeros(nb, POSE_DTYPE); upd = np.zeros(nb, np.uint32)
+    ctx.check(L.cvb_single_view_optimize_l1(ctx.handle, p.ctypes.data, nb, epsilon, optimization_rate, iterations, b.ctypes.data,
+                                            w.ctypes.data, off.ctypes.data, out.ctypes.data, upd.ctypes.data))
+    return _poses_out(out), upd
+
+
+def single_view_simple_optimize_l1(pose, epsilon, optimization_rate, iterations, landmarks, ctx=None):
+    """landmarks = (bearings[n,3], world[n,4]) FeatureWorldMatches -> refined (R, t); the reference's Weiszfeld iteration, epsilon
+    has no default there either"""
+    bearings, world = landmarks
+    if len(bearings) == 0:
+        return pose
+    out, _ = single_view_simple_optimize_l1_batch([pose], epsilon, optimization_rate, iterations, bearings, world, [0, len(bearings)], ctx)
+    return out[0]
+
+
+def three_view_simple_optimize_l1_batch(poses, epsilon, optimization_rate, iterations, observations, offsets, ctx=None):
+    """B problems of three_view_simple_optimize_l1: poses[b] = [(R, t) centre->first, (R, t) centre->second];
+    observations[n,3,3] = (centre, first, second) bearings -> ([[(R, t), (R, t)]], updates[B])"""
+    ctx, L = _l1_lib(ctx)
+    flat = [q for pair in poses for q in pair]
+    p = _poses_in(flat)
+    o = np.ascontiguousarray(observations, np.float64).reshape(-1, 9)
+    off = np.ascontiguousarray(offsets, np.uint32)
+    nb = len(off) - 1
+    if 2 * nb != len(p) or off[-1] != len(o):
+        raise ValueError("offsets / poses / observation arrays disagree")
+    out = np.zeros(2 * nb, POSE_DTYPE); upd = np.zeros(nb, np.uint32)
+    ctx.check(L.cvb_three_view_optimize_l1(ctx.handle, p.ctypes.data, nb, epsilon, optimization_rate, iterations, o.ctypes.data,
+                                           off.ctypes.data, out.ctypes.data, upd.ctypes.data))
+    po = _poses_out(out)
+    return [[po[2 * i], po[2 * i + 1]] for i in range(nb)], upd
+
+
+def three_view_simple_optimize_l1(poses, epsilon, optimization_rate, iterations, landmarks, ctx=None):
+    if len(landmarks) == 0:
+        return list(poses)
+    return three_view_simple_optimize_l1_batch([poses], epsilon, optimization_rate, iterations, landmarks, [0, len(landmarks)], ctx)[0][0]
 
 
 def observation_losses(poses, bearings, offsets, ctx=None, triangulator=None):
