@@ -186,3 +186,6 @@ pub use tri::*;
 
 // ---- INTEGRATION.md section 2e (include/cvb200_opt.h) ----
 pub mod opt;
+
+// ---- INTEGRATION.md section 2f (include/cvb200_pinhole.h) ----
+pub mod pinhole;

@@ -7,6 +7,7 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   LinearKnn / hamming_knn <- space::LinearKnn + bitarray::Hamming (call sites akaze/tests/estimate_pose.rs:78-97)
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
   CameraIntrinsics(K1Distortion) <- cv-pinhole/src/lib.rs:32-240
+  *pose_reprojection_error, EssentialMatrix <- cv-pinhole/src/lib.rs:314-372, essential.rs:56-275
   frame_features        <- cv-sfm VSlam::kps_descriptors        (cv-sfm/src/lib.rs:2195-2235)
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
@@ -17,7 +18,8 @@ CvbError when the library or a Hopper (sm_90) GPU is missing.
 from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F401
 from .akaze import Akaze, AkazeConfig  # noqa: F401
 from .knn import HammingHasher, LinearKnn, hamming_knn, lowe_ratio_matches, matching, symmetric_matching  # noqa: F401
-from .pinhole import CameraIntrinsics, CameraIntrinsicsK1Distortion  # noqa: F401
+from .pinhole import (CameraIntrinsics, CameraIntrinsicsK1Distortion, EssentialMatrix, average_pose_reprojection_error,  # noqa: F401
+                      average_pose_reprojection_error_batch, pose_reprojection_error, pose_reprojection_error_batch)
 from .geom import (Arrsac, EightPoint, LambdaTwist, NisterStewenius, Pcg64, Xoshiro256PlusPlus,  # noqa: F401
                    residuals_camera_to_camera, residuals_world_to_camera)
 from .triangulation import (AngularL1Triangulator, AngularLInfinityTriangulator, LinearEigenTriangulator,  # noqa: F401

@@ -1,5 +1,5 @@
-"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its module
-cv_b200/libcvb200_opt.so (include/cvb200_opt.h)."""
+"""ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
+cv_b200/libcvb200_opt.so (include/cvb200_opt.h) and cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h)."""
 import ctypes as C
 import os
 
@@ -69,6 +69,13 @@ TRI_ABI_SYMBOLS = [
 # every symbol include/cvb200_opt.h declares (cv-optimize's L1 optimizers), exported by libcvb200_opt.so; checked by tests/test_abi_opt.py
 OPT_ABI_SYMBOLS = [
     "cvb_single_view_optimize_l1", "cvb_three_view_optimize_l1",
+]
+
+# every symbol include/cvb200_pinhole.h declares (cv-pinhole's reprojection error and EssentialMatrix), exported by libcvb200_pinhole.so;
+# checked by tests/test_abi_pinhole.py
+PINHOLE_ABI_SYMBOLS = [
+    "cvb_pose_reprojection_error", "cvb_pose_reprojection_error_dev", "cvb_eight_point_essential_batch", "cvb_residuals_essential",
+    "cvb_essential_recondition", "cvb_essential_decompose",
 ]
 
 
@@ -142,6 +149,25 @@ def load_opt_library():
             raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
         _OPT_LIB = C.CDLL(p)
     return _OPT_LIB
+
+
+_PINHOLE_LIB = None
+
+
+def pinhole_lib_path():
+    return os.path.join(_HERE, "libcvb200_pinhole.so")
+
+
+def load_pinhole_library():
+    """Loads libcvb200_pinhole.so, the module of include/cvb200_pinhole.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _PINHOLE_LIB
+    if _PINHOLE_LIB is None:
+        load_library()
+        p = pinhole_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        _PINHOLE_LIB = C.CDLL(p)
+    return _PINHOLE_LIB
 
 
 class Context:

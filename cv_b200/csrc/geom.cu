@@ -15,6 +15,7 @@
 #include "common.cuh"
 #include "../../include/cvb200_tri.h"
 #include "../../include/cvb200_opt.h"
+#include "../../include/cvb200_pinhole.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -152,8 +153,8 @@ __device__ __forceinline__ double det3(const double *m) {
 }
 
 // sorted SVD of a 3x3 matrix through the eigen-decomposition of MtM; u3 = u1 x u2 (its sign is normalised by
-// the det(U) > 0 rule of essential.rs:139-143 anyway)
-__device__ __noinline__ bool svd3(const double *M, double eps, int iters, double *U, double *Vt) {
+// the det(U) > 0 rule of essential.rs:139-143 anyway).  S (may be null) receives the singular values, descending.
+__device__ __noinline__ bool svd3(const double *M, double eps, int iters, double *U, double *Vt, double *S = nullptr) {
     double MtM[9], d[3], V[9];
     for (int i = 0; i < 3; i++)
         for (int j = 0; j < 3; j++) MtM[i * 3 + j] = M[i] * M[j] + M[3 + i] * M[3 + j] + M[6 + i] * M[6 + j];
@@ -178,6 +179,7 @@ __device__ __noinline__ bool svd3(const double *M, double eps, int iters, double
     for (int r = 0; r < 3; r++) u[2][r] /= nn;
     for (int k = 0; k < 3; k++)
         for (int r = 0; r < 3; r++) { U[r * 3 + k] = u[k][r]; Vt[k * 3 + r] = v[k][r]; }
+    if (S) for (int k = 0; k < 3; k++) S[k] = s[k];
     return true;
 }
 
@@ -686,17 +688,24 @@ __device__ void fp_o2(const double *a, const double *b, double *r) {
     r[B1] = a[B1] * b[3];
 }
 
-// essential matrix -> the four candidate poses (cv-pinhole/src/essential.rs:114-162,217-231)
-__device__ __noinline__ int essential_poses(const double *E, cvb_pose *out) {
+// EssentialMatrix::possible_rotations_unscaled_translation (cv-pinhole/src/essential.rs:114-162): Ra = U W Vt, Rb = U Wt Vt and
+// t = U's third column, after the det(U), det(Vt) > 0 fix-ups
+__device__ __noinline__ bool essential_rotations(const double *E, double eps, int sweeps, double *Ra, double *Rb, double *t) {
     double U[9], Vt[9];
-    if (!svd3(E, 1e-12, 1000, U, Vt)) return 0;
+    if (!svd3(E, eps, sweeps, U, Vt)) return false;
     if (det3(U) < 0.0) for (int r = 0; r < 3; r++) U[r * 3 + 2] *= -1.0;
     if (det3(Vt) < 0.0) for (int c = 0; c < 3; c++) Vt[6 + c] *= -1.0;
     const double W[9] = {0, -1, 0, 1, 0, 0, 0, 0, 1}, Wt[9] = {0, 1, 0, -1, 0, 0, 0, 0, 1};
-    double UW[9], Ra[9], Rb[9];
+    double UW[9];
     mat3_mul(U, W, UW); mat3_mul(UW, Vt, Ra);
     mat3_mul(U, Wt, UW); mat3_mul(UW, Vt, Rb);
-    const double t[3] = {U[2], U[5], U[8]};
+    t[0] = U[2]; t[1] = U[5]; t[2] = U[8];
+    return true;
+}
+// essential matrix -> the four candidate poses (cv-pinhole/src/essential.rs:114-162,217-231) with Estimator::estimate's 1e-12 / 1000
+__device__ __noinline__ int essential_poses(const double *E, cvb_pose *out) {
+    double Ra[9], Rb[9], t[3];
+    if (!essential_rotations(E, 1e-12, 1000, Ra, Rb, t)) return 0;
     for (int k = 0; k < 4; k++) {
         for (int i = 0; i < 9; i++) out[k].r[i] = (k & 1) ? Rb[i] : Ra[i];
         for (int r = 0; r < 3; r++) out[k].t[r] = (k & 2) ? -t[r] : t[r];
@@ -1420,6 +1429,15 @@ __device__ bool triangulate_angular(bool linf, const cvb_pose &P, const double *
     if (!finite4(p)) return false;
     return !signbit(dot3(p, a)) && !signbit(dot3(p, b));
 }
+// TriangulatorRelative::triangulate_relative of all six methods
+__device__ __forceinline__ bool triangulate_relative(const cvb_triangulator &T, const cvb_pose &P, const double *a, const double *b, double *p) {
+    switch (T.method) {
+    case CVB_TRI_RELATIVE_DLT: return triangulate_relative_dlt(T, P, a, b, p);
+    case CVB_TRI_ANGULAR_L1: return triangulate_angular(false, P, a, b, p);
+    case CVB_TRI_ANGULAR_LINF: return triangulate_angular(true, P, a, b, p);
+    default: return triangulate_relative_obs(T, P, a, b, p);
+    }
+}
 // one thread per (relative pose, a, b) triple; npose = 1 shares poses[0]
 __global__ void __launch_bounds__(128) k_triangulate_relative(cvb_triangulator T, const cvb_pose *__restrict__ poses, uint32_t npose,
                                                               const double *__restrict__ a, const double *__restrict__ b, uint32_t n,
@@ -1429,13 +1447,7 @@ __global__ void __launch_bounds__(128) k_triangulate_relative(cvb_triangulator T
     const cvb_pose P = poses[npose == 1 ? 0 : i];
     const double *ai = a + 3 * (size_t)i, *bi = b + 3 * (size_t)i;
     double p[4] = {0, 0, 0, 0};
-    bool good;
-    switch (T.method) {
-    case CVB_TRI_RELATIVE_DLT: good = triangulate_relative_dlt(T, P, ai, bi, p); break;
-    case CVB_TRI_ANGULAR_L1: good = triangulate_angular(false, P, ai, bi, p); break;
-    case CVB_TRI_ANGULAR_LINF: good = triangulate_angular(true, P, ai, bi, p); break;
-    default: good = triangulate_relative_obs(T, P, ai, bi, p);
-    }
+    const bool good = triangulate_relative(T, P, ai, bi, p);
     ok[i] = good ? 1 : 0;
     for (int k = 0; k < 4; k++) xyzw[(size_t)i * 4 + k] = good ? p[k] : 0.0;
 }
@@ -1488,6 +1500,113 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
         && transformed_cosine_distance(second, p, s) < max_cos;
     const bool incidence_ok = 1.0 - dot3(c, fc) > inc_min_cos || 1.0 - dot3(c, sc) > inc_min_cos || 1.0 - dot3(fc, sc) > inc_min_cos;
     out[i] = cosine_ok && incidence_ok;
+}
+
+// ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
+// cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
+//  - a_norm = a.xy / a.z and b_norm = b.xy / b.z come from the INPUT bearings (:320-321);
+//  - the triangulated CameraPoint's bearing is its xyz (Projective::bearing, cv-core/src/point.rs:46-49), reprojected only when
+//    bearing.z.is_sign_positive() -- a sign-bit test, so +0.0 and +NaN pass and their infinities / NaNs reach the error (:325-328);
+//  - point_b = pose.transform(point_a) = from_homogeneous([R xyz + t w; w]) with the same test on its bearing (:329-334);
+//  - average = ((0 + |e_a|) + |e_b|) * 0.5 with |v| = sqrt(x x + y y) (:370-371).
+// the value of a row the reference returns None for: the quiet NaN of C's NAN and numpy's nan (CUDART_NAN has the sign bit set)
+__device__ __forceinline__ double none_nan() { return __longlong_as_double(0x7ff8000000000000ull); }
+__device__ bool pose_reprojection(const cvb_triangulator &T, const cvb_pose &P, const double *a, const double *b, double *e, double *avg) {
+    const double an[2] = {a[0] / a[2], a[1] / a[2]}, bn[2] = {b[0] / b[2], b[1] / b[2]};
+    double p[4] = {0, 0, 0, 0}, q[4];
+    if (!triangulate_relative(T, P, a, b, p)) return false;
+    if (signbit(p[2])) return false;
+    pose_apply(P, p, q);
+    from_homogeneous(q);
+    if (signbit(q[2])) return false;
+    e[0] = an[0] - p[0] / p[2]; e[1] = an[1] - p[1] / p[2];
+    e[2] = bn[0] - q[0] / q[2]; e[3] = bn[1] - q[1] / q[2];
+    *avg = ((0.0 + sqrt(e[0] * e[0] + e[1] * e[1])) + sqrt(e[2] * e[2] + e[3] * e[3])) * 0.5;
+    return true;
+}
+// one thread per match; rows i < min(*n_dev, n) (n_dev null: n) are written; found (may be null) == 0 marks every row as None
+__global__ void __launch_bounds__(128) k_pose_reprojection_error(cvb_triangulator T, const cvb_pose *__restrict__ poses, uint32_t npose,
+                                                                 const double *__restrict__ a, const double *__restrict__ b,
+                                                                 const uint32_t *__restrict__ n_dev, uint32_t n, const int32_t *__restrict__ found,
+                                                                 double *__restrict__ err, double *__restrict__ avg, uint8_t *__restrict__ ok) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (n_dev ? min(*n_dev, n) : n)) return;
+    double e[4], m;
+    const bool good = (!found || *found != 0) &&
+                      pose_reprojection(T, poses[npose == 1 ? 0 : i], a + 3 * (size_t)i, b + 3 * (size_t)i, e, &m);
+    ok[i] = good ? 1 : 0;
+    for (int k = 0; k < 4; k++) err[(size_t)i * 4 + k] = good ? e[k] : none_nan();
+    if (avg) avg[i] = good ? m : none_nan();
+}
+
+// EightPoint { epsilon, iterations }::from_matches (eight-point/src/lib.rs:43-58) on one sample of 8 matches: the design rows, Gram
+// matrix and round-robin Jacobi of eight_point(), with the caller's epsilon and sweep bound
+__global__ void __launch_bounds__(128) k_eight_point_essential(const double *__restrict__ a, const double *__restrict__ b,
+                                                               const uint32_t *__restrict__ samples, uint32_t H, double eps, int sweeps,
+                                                               double *__restrict__ E_out, uint8_t *__restrict__ ok) {
+    const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= H) return;
+    double D[72], EtE[81], V[81];
+    for (int i = 0; i < 8; i++) eight_point_row(a, b, samples[(size_t)h * 8 + i], D + 9 * i);
+    for (int r = 0; r < 9; r++)
+        for (int c = 0; c < 9; c++) EtE[r * 9 + c] = eight_point_gram(D, r, c);
+    const bool good = sym_eigen9_rr<1>(EtE, V, 0, 0u, eps, sweeps);
+    int best = 0;
+    for (int i = 1; i < 9; i++)
+        if (EtE[i * 9 + i] < EtE[best * 9 + best]) best = i;
+    double *E = E_out + (size_t)h * 9;
+    for (int k = 0; k < 9; k++) E[(k % 3) * 3 + (k / 3)] = good ? V[k * 9 + best] : none_nan();   // Matrix3::from_iterator: column-major
+    ok[h] = good ? 1 : 0;
+}
+
+// cv-pinhole/src/essential.rs:266-275 EssentialMatrix::residual as |nb . (E na)|: E na first, then the dot product with nb (nalgebra's
+// b^T E a groups (b^T E) a, so the last bit can differ from the reference; the CPU restatement groups it this way too)
+__device__ __forceinline__ double residual_essential(const double *E, const double *a, const double *b) {
+    const double na[3] = {a[0] / a[2], a[1] / a[2], a[2] / a[2]}, nb[3] = {b[0] / b[2], b[1] / b[2], b[2] / b[2]};
+    const double Ea[3] = {dot3(E, na), dot3(E + 3, na), dot3(E + 6, na)};
+    return fabs(dot3(nb, Ea));
+}
+// one thread per (E, datum), the layout of k_residuals
+__global__ void __launch_bounds__(256) k_residuals_essential(const double *__restrict__ Es, const double *__restrict__ a,
+                                                             const double *__restrict__ b, uint32_t n, double *__restrict__ out) {
+    const uint32_t p = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    double E[9];
+    for (int k = 0; k < 9; k++) E[k] = Es[(size_t)p * 9 + k];
+    out[(size_t)p * n + i] = residual_essential(E, a + 3 * (size_t)i, b + 3 * (size_t)i);
+}
+
+// cv-pinhole/src/essential.rs:64-77 EssentialMatrix::recondition: SVD::recompose of U diag(s, s, 0) Vt, s = (s0 + s1) / 2 (nalgebra
+// scales U's columns, then multiplies by Vt); one thread per matrix
+__global__ void __launch_bounds__(128) k_essential_recondition(const double *__restrict__ Es, uint32_t m, double eps, int sweeps,
+                                                               double *__restrict__ E_out, uint8_t *__restrict__ ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    double E[9], U[9], Vt[9], S[3], R[9];
+    for (int k = 0; k < 9; k++) E[k] = Es[(size_t)j * 9 + k];
+    const bool good = svd3(E, eps, sweeps, U, Vt, S);
+    if (good) {
+        const double s = (S[0] + S[1]) / 2.0, d[3] = {s, s, 0.0};
+        for (int r = 0; r < 3; r++)
+            for (int c = 0; c < 3; c++) U[r * 3 + c] *= d[c];
+        mat3_mul(U, Vt, R);
+    }
+    for (int k = 0; k < 9; k++) E_out[(size_t)j * 9 + k] = good ? R[k] : none_nan();
+    ok[j] = good ? 1 : 0;
+}
+
+// cv-pinhole/src/essential.rs:114-162 possible_rotations_unscaled_translation; one thread per matrix
+__global__ void __launch_bounds__(128) k_essential_decompose(const double *__restrict__ Es, uint32_t m, double eps, int sweeps,
+                                                             double *__restrict__ rot_a, double *__restrict__ rot_b, double *__restrict__ t_out,
+                                                             uint8_t *__restrict__ ok) {
+    const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= m) return;
+    double E[9], Ra[9], Rb[9], t[3];
+    for (int k = 0; k < 9; k++) E[k] = Es[(size_t)j * 9 + k];
+    const bool good = essential_rotations(E, eps, sweeps, Ra, Rb, t);
+    for (int k = 0; k < 9; k++) { rot_a[(size_t)j * 9 + k] = good ? Ra[k] : none_nan(); rot_b[(size_t)j * 9 + k] = good ? Rb[k] : none_nan(); }
+    for (int k = 0; k < 3; k++) t_out[(size_t)j * 3 + k] = good ? t[k] : none_nan();
+    ok[j] = good ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -2601,6 +2720,153 @@ int opt_three_view_l1(cvb_ctx *ctx, const cvb_pose *poses, uint32_t B, double ep
         CVB_LAUNCH_CHECK(ctx);
     }
     return download_poses_updates(ctx, g, poses_out, 2 * (size_t)B, updates_out, B);
+}
+
+// The entry points of include/cvb200_pinhole.h, exported by libcvb200_pinhole.so (cv_b200/csrc/pinhole_abi.cu) for the same reason.
+// max_iterations (usize upstream) as the Jacobi sweep bound, as tri_sweeps does for the triangulators
+static int pinhole_sweeps(uint32_t max_iterations) { return max_iterations > 0x7fffffffu ? 0x7fffffff : (int)max_iterations; }
+
+int pin_pose_reprojection_error(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses, uint32_t npose, const double *a,
+                                const double *b, uint32_t n, double *err_out, double *avg_out, uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, true))) return rc;
+    if (n == 0) return 0;
+    if (npose != 1 && npose != n) return cvb_set_error(ctx, CVB_EINVAL, "npose must be 1 or n (%u), not %u", n, npose);
+    if (!poses || !a || !b || !err_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = upload(ctx, g->poses, poses, sizeof(cvb_pose) * (size_t)npose))) return rc;
+    if ((rc = upload(ctx, g->a, a, sizeof(double) * 3 * (size_t)n))) return rc;
+    if ((rc = upload(ctx, g->b, b, sizeof(double) * 3 * (size_t)n))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * 5 * (size_t)n))) return rc;   // err (n x 4) | avg (n)
+    if ((rc = g->ok.ensure(ctx, n))) return rc;
+    double *err = (double *)g->out.p, *avg = err + 4 * (size_t)n;
+    {
+        CVB_PROF(ctx, "k_pose_reprojection_error", 89.0 * n + sizeof(cvb_pose) * (double)npose);
+        k_pose_reprojection_error<<<cdiv(n, 128), 128, 0, ctx->stream>>>(*tri, (const cvb_pose *)g->poses.p, npose, (const double *)g->a.p,
+                                                                         (const double *)g->b.p, nullptr, n, nullptr, err, avg, (uint8_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(err_out, err, sizeof(double) * 4 * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    if (avg_out) CVB_CUDA(ctx, cudaMemcpyAsync(avg_out, avg, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, n, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int pin_pose_reprojection_error_dev(cvb_ctx *ctx, const cvb_triangulator *tri, const cvb_pose *poses_dev, uint32_t npose,
+                                    const double *a_dev, const double *b_dev, const uint32_t *n_dev, uint32_t n_max,
+                                    const int32_t *found_dev, double *err_out_dev, double *avg_out_dev, uint8_t *ok_out_dev) {
+    if (!ctx) return CVB_EINVAL;
+    int rc;
+    if ((rc = tri_check(ctx, tri, true))) return rc;
+    if (npose != 1 && npose != n_max) return cvb_set_error(ctx, CVB_EINVAL, "npose must be 1 or n_max (%u), not %u", n_max, npose);
+    if (!poses_dev || !a_dev || !b_dev || !n_dev || !err_out_dev || !ok_out_dev) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (n_max == 0) return 0;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    CVB_PROF(ctx, "k_pose_reprojection_error", 0);
+    k_pose_reprojection_error<<<cdiv(n_max, 128), 128, 0, ctx->stream>>>(*tri, poses_dev, npose, a_dev, b_dev, n_dev, n_max, found_dev,
+                                                                         err_out_dev, avg_out_dev, ok_out_dev);
+    CVB_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+int pin_eight_point_essential_batch(cvb_ctx *ctx, double epsilon, uint32_t iterations, const double *a, const double *b, uint32_t n,
+                                    const uint32_t *samples, uint32_t H, double *E_out, uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (H == 0) return 0;
+    if (!a || !b || !samples || !E_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    for (size_t i = 0; i < (size_t)H * 8; i++)
+        if (samples[i] >= n) return cvb_set_error(ctx, CVB_EINVAL, "sample index %u out of range (n = %u)", samples[i], n);
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = upload_data(ctx, 0, a, b, n))) return rc;
+    if ((rc = upload(ctx, g->samples, samples, sizeof(uint32_t) * 8 * (size_t)H))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * 9 * (size_t)H))) return rc;
+    if ((rc = g->ok.ensure(ctx, H))) return rc;
+    {
+        CVB_PROF(ctx, "k_eight_point_essential", 0);
+        k_eight_point_essential<<<cdiv(H, 128), 128, 0, ctx->stream>>>((const double *)g->a.p, (const double *)g->b.p, (const uint32_t *)g->samples.p,
+                                                                       H, epsilon, pinhole_sweeps(iterations), (double *)g->out.p, (uint8_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(E_out, g->out.p, sizeof(double) * 9 * (size_t)H, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, H, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int pin_residuals_essential(cvb_ctx *ctx, const double *E, uint32_t m, const double *a, const double *b, uint32_t n, double *out) {
+    if (!ctx) return CVB_EINVAL;
+    if (m == 0 || n == 0) return 0;
+    if (!E || !a || !b || !out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = upload_data(ctx, 0, a, b, n))) return rc;
+    if ((rc = upload(ctx, g->poses, E, sizeof(double) * 9 * (size_t)m))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * (size_t)m * n))) return rc;
+    for (uint32_t p0 = 0; p0 < m; p0 += 65535) {   // gridDim.y limit
+        const uint32_t pm = std::min<uint32_t>(65535, m - p0);
+        CVB_PROF(ctx, "k_residuals_essential", 56.0 * pm * n);
+        k_residuals_essential<<<dim3(cdiv(n, 256), pm), 256, 0, ctx->stream>>>((const double *)g->poses.p + (size_t)p0 * 9, (const double *)g->a.p,
+                                                                               (const double *)g->b.p, n, (double *)g->out.p + (size_t)p0 * n);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(out, g->out.p, sizeof(double) * (size_t)m * n, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int pin_essential_recondition(cvb_ctx *ctx, const double *E, uint32_t m, double epsilon, uint32_t max_iterations, double *E_out,
+                              uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (m == 0) return 0;
+    if (!E || !E_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = upload(ctx, g->poses, E, sizeof(double) * 9 * (size_t)m))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * 9 * (size_t)m))) return rc;
+    if ((rc = g->ok.ensure(ctx, m))) return rc;
+    {
+        CVB_PROF(ctx, "k_essential_recondition", 144.0 * m);
+        k_essential_recondition<<<cdiv(m, 128), 128, 0, ctx->stream>>>((const double *)g->poses.p, m, epsilon, pinhole_sweeps(max_iterations),
+                                                                       (double *)g->out.p, (uint8_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(E_out, g->out.p, sizeof(double) * 9 * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int pin_essential_decompose(cvb_ctx *ctx, const double *E, uint32_t m, double epsilon, uint32_t max_iterations, double *rot_a_out,
+                            double *rot_b_out, double *t_out, uint8_t *ok_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (m == 0) return 0;
+    if (!E || !rot_a_out || !rot_b_out || !t_out || !ok_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = upload(ctx, g->poses, E, sizeof(double) * 9 * (size_t)m))) return rc;
+    if ((rc = g->out.ensure(ctx, sizeof(double) * 21 * (size_t)m))) return rc;   // rot_a (m x 9) | rot_b (m x 9) | t (m x 3)
+    if ((rc = g->ok.ensure(ctx, m))) return rc;
+    double *ra = (double *)g->out.p, *rb = ra + 9 * (size_t)m, *t = rb + 9 * (size_t)m;
+    {
+        CVB_PROF(ctx, "k_essential_decompose", 240.0 * m);
+        k_essential_decompose<<<cdiv(m, 128), 128, 0, ctx->stream>>>((const double *)g->poses.p, m, epsilon, pinhole_sweeps(max_iterations),
+                                                                     ra, rb, t, (uint8_t *)g->ok.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(rot_a_out, ra, sizeof(double) * 9 * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(rot_b_out, rb, sizeof(double) * 9 * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(t_out, t, sizeof(double) * 3 * (size_t)m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(ok_out, g->ok.p, m, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
 }
 
 extern "C" {

@@ -127,6 +127,15 @@ class EightPoint:
         poses, cnt = self.estimate_batch(a, b, np.arange(8, dtype=np.uint32)[None], ctx)
         return [(poses[0, k]["r"].reshape(3, 3).copy(), poses[0, k]["t"].copy()) for k in range(cnt[0])]
 
+    def from_matches(self, a, b, epsilon=1e-12, iterations=1000, ctx=None):
+        """EightPoint { epsilon, iterations }::from_matches (eight-point/src/lib.rs:43-58) on the first 8 matches -> EssentialMatrix or
+        None.  To recondition the result, see EssentialMatrix.recondition.  Batched over samples: cv_b200.pinhole.eight_point_essential_batch."""
+        from .pinhole import EssentialMatrix, eight_point_essential_batch
+        if len(a) < 8:
+            raise ValueError("from_matches needs 8 matches")
+        E, ok = eight_point_essential_batch(a, b, np.arange(8, dtype=np.uint32)[None], epsilon, iterations, ctx)
+        return EssentialMatrix(E[0]) if ok[0] else None
+
 
 class NisterStewenius:
     """nister_stewenius::NisterStewenius: MIN_SAMPLES = 5, up to 40 CameraToCamera poses per sample
