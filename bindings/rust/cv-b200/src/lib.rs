@@ -6,7 +6,7 @@ use std::{ffi::CStr, sync::Arc};
 
 use bitarray::{BitArray, Hamming};
 use cv_b200_sys::*;
-use image::DynamicImage;
+use ::image::DynamicImage;      // the image crate (the sys crate's module `image` is glob-imported above)
 use space::Neighbor;
 
 /// One library context (CUDA stream + workspaces).  Not thread-safe: keep one per worker thread; clones share the handle.
@@ -189,3 +189,6 @@ pub mod opt;
 
 // ---- INTEGRATION.md section 2f (include/cvb200_pinhole.h) ----
 pub mod pinhole;
+
+// ---- INTEGRATION.md section 2g (include/cvb200_image.h) ----
+pub mod dynamic;

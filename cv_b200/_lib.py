@@ -1,5 +1,6 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
-cv_b200/libcvb200_opt.so (include/cvb200_opt.h) and cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h)."""
+cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h) and cv_b200/libcvb200_image.so
+(include/cvb200_image.h)."""
 import ctypes as C
 import os
 
@@ -76,6 +77,13 @@ OPT_ABI_SYMBOLS = [
 PINHOLE_ABI_SYMBOLS = [
     "cvb_pose_reprojection_error", "cvb_pose_reprojection_error_dev", "cvb_eight_point_essential_batch", "cvb_residuals_essential",
     "cvb_essential_recondition", "cvb_essential_decompose",
+]
+
+# every symbol include/cvb200_image.h declares (8- and 16-bit frames into the extractor), exported by libcvb200_image.so;
+# checked by tests/test_abi_image.py
+IMAGE_ABI_SYMBOLS = [
+    "cvb_gray_float_from_dynamic_dev", "cvb_akaze_extract_dynamic_batch", "cvb_akaze_extract_dynamic_batch_dev",
+    "cvb_frame_features_dynamic_batch", "cvb_two_view_frames_dynamic_k1",
 ]
 
 
@@ -168,6 +176,25 @@ def load_pinhole_library():
             raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
         _PINHOLE_LIB = C.CDLL(p)
     return _PINHOLE_LIB
+
+
+_IMAGE_LIB = None
+
+
+def image_lib_path():
+    return os.path.join(_HERE, "libcvb200_image.so")
+
+
+def load_image_library():
+    """Loads libcvb200_image.so, the module of include/cvb200_image.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _IMAGE_LIB
+    if _IMAGE_LIB is None:
+        load_library()
+        p = image_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        _IMAGE_LIB = C.CDLL(p)
+    return _IMAGE_LIB
 
 
 class Context:

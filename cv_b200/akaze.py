@@ -5,6 +5,9 @@ from dataclasses import dataclass
 import numpy as np
 
 from ._lib import KP_DTYPE, AkazeCfg, Context, CvbError, default_context
+from .image import DynamicImage, is_dynamic
+from .image import lib as _image_lib
+from .image import stack as _stack_frames
 
 PLANES = {"Lt": 0, "Lsmooth": 1, "Lx": 2, "Ly": 3, "Lflow": 4, "Ldet": 5}
 STAGES = {"candidates": 0, "extrema": 1, "refined": 2, "sorted": 3}
@@ -57,6 +60,11 @@ class Akaze:
 
     # -- Akaze::extract (lib.rs:295): DynamicImage -> GrayFloatImage::from_dynamic (image.rs:45-109)
     def extract(self, image):
+        """A DynamicImage is converted on the device (include/cvb200_image.h); a numpy array is converted here: uint8 / 255,
+        uint16 / 65535, float32 as it is, [H, W] only."""
+        if isinstance(image, DynamicImage):
+            kps, descs = self.extract_batch([image])
+            return kps[0], descs[0]
         image = np.asarray(image)
         if image.dtype == np.uint8:
             f = image.astype(np.float32) / np.float32(255)
@@ -76,7 +84,10 @@ class Akaze:
         return kps[0], descs[0]
 
     def extract_batch(self, images):
-        """B independent frames of one size in a single pass. Returns lists of (keypoints, descriptors)."""
+        """B independent frames of one size in a single pass: [B, H, W] float32, or a list of DynamicImage of one size and format
+        (uploaded as they are and converted on the device).  Returns lists of (keypoints, descriptors)."""
+        if is_dynamic(images):
+            return self._extract_dynamic(images)
         images = np.ascontiguousarray(images, dtype=np.float32)
         if images.ndim != 3:
             raise ValueError("images must be [B, H, W] float32")
@@ -90,6 +101,20 @@ class Akaze:
         rc = ctx.lib.cvb_akaze_extract_batch(ctx.handle, C.byref(cfg), images.ctypes.data, B, W, H, kp.ctypes.data,
                                              desc.ctypes.data, cap, n.ctypes.data)
         ctx.check(rc)
+        return [kp[b, :n[b]].copy() for b in range(B)], [desc[b, :n[b]].copy() for b in range(B)]
+
+    def _extract_dynamic(self, images):
+        fmt, pixels, W, H = _stack_frames(images)
+        B = pixels.shape[0]
+        ctx = self._ctx()
+        L = _image_lib()
+        cap = self.max_keypoints
+        kp = np.zeros((B, cap), dtype=KP_DTYPE)
+        desc = np.zeros((B, cap, 64), dtype=np.uint8)
+        n = np.zeros(B, dtype=np.uint32)
+        cfg = self.config.to_c()
+        ctx.check(L.cvb_akaze_extract_dynamic_batch(ctx.handle, C.byref(cfg), fmt, pixels.ctypes.data, B, W, H, kp.ctypes.data,
+                                                    desc.ctypes.data, cap, n.ctypes.data))
         return [kp[b, :n[b]].copy() for b in range(B)], [desc[b, :n[b]].copy() for b in range(B)]
 
     # -- introspection used by the parity tests (no reference counterpart)

@@ -862,6 +862,13 @@ int cvb_akaze_dev_overflow(cvb_ctx *ctx, uint32_t *flag_out) {
 
 int cvb_akaze_extract_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, uint32_t batch, uint32_t w, uint32_t h,
                             cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out) {
+    return akaze_extract_batch_host(ctx, cfg, images, false, batch, w, h, kp_out, desc_out, cap, n_out);
+}
+
+}  // extern "C"
+
+int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, bool images_on_device, uint32_t batch, uint32_t w,
+                             uint32_t h, cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out) {
     int rc = check_args(ctx, cfg, images, batch, w, h);
     if (rc) return rc;
     if (!n_out || (cap && (!kp_out || !desc_out))) return cvb_set_error(ctx, CVB_EINVAL, "null output");
@@ -870,9 +877,9 @@ int cvb_akaze_extract_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float 
     if (rc) return rc;
     AkazeWorkspace *ws = ctx->akaze;
     cudaStream_t st = ctx->stream;
-    CVB_CUDA(ctx, cudaMemcpyAsync(ws->img, images, sizeof(float) * ws->p0 * batch, cudaMemcpyHostToDevice, st));
+    if (!images_on_device) CVB_CUDA(ctx, cudaMemcpyAsync(ws->img, images, sizeof(float) * ws->p0 * batch, cudaMemcpyHostToDevice, st));
     const unsigned cap_dev = ws->cap_out;
-    rc = run_extract(ctx, ws->img, batch, ws->kp_out, ws->desc_out, cap_dev, ws->n_out);
+    rc = run_extract(ctx, images_on_device ? images : ws->img, batch, ws->kp_out, ws->desc_out, cap_dev, ws->n_out);
     if (rc) return rc;
     unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * ((size_t)batch + 1));
     if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
@@ -897,6 +904,8 @@ int cvb_akaze_extract_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float 
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
+
+extern "C" {
 
 int cvb_akaze_extract(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *image, uint32_t w, uint32_t h, cvb_keypoint *kp_out,
                       uint8_t *desc_out, uint32_t cap, uint32_t *n_out) {

@@ -11,6 +11,7 @@ struct MatchWorkspace;
 struct GeomWorkspace;
 struct PairWorkspace;
 struct FrameWorkspace;
+struct ImageWorkspace;
 
 struct cvb_ctx {
     int device = 0;
@@ -26,6 +27,7 @@ struct cvb_ctx {
     GeomWorkspace *geom = nullptr;
     PairWorkspace *pair = nullptr;
     FrameWorkspace *frame = nullptr;
+    ImageWorkspace *image = nullptr;
     // page-locked host scratch for the small device->host results of the host API (a D2H copy into pageable memory is
     // staged synchronously inside the driver and stalls the other contexts' launches)
     void *pinned = nullptr;
@@ -61,6 +63,20 @@ void match_workspace_free(MatchWorkspace *ws);
 void geom_workspace_free(GeomWorkspace *ws);
 void pair_workspace_free(PairWorkspace *ws);
 void frame_workspace_free(FrameWorkspace *ws);
+void image_workspace_free(ImageWorkspace *ws);
+
+// Bodies of the host-API entry points cvb_akaze_extract_batch, cvb_frame_features_batch and cvb_two_view_frames_k1.  With the
+// *_on_device flag set, the f32 planes (and the RGB8 plane) are already on the device and nothing is uploaded: the pixel-format entry
+// points of image.cu (include/cvb200_image.h) convert into their own buffers, then take exactly these paths.
+int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, bool images_on_device, uint32_t batch, uint32_t w,
+                             uint32_t h, cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out);
+int frame_features_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, const uint8_t *rgb, bool planes_on_device,
+                              uint32_t batch, uint32_t w, uint32_t h, const cvb_intrinsics_k1 *intrinsics, cvb_keypoint *kp_out,
+                              uint8_t *desc_out, double *bearings_out, uint8_t *colors_out, uint32_t cap, uint32_t *n_out);
+int two_view_frames_k1_host(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *frames, bool frames_on_device, uint32_t w, uint32_t h,
+                            uint32_t better_by, const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng,
+                            cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs,
+                            cvb_pose *model_out, uint32_t *inliers_out, uint32_t *n_inliers, int32_t *found);
 
 #define CVB_CUDA(ctx, call)                                                                          \
     do {                                                                                             \

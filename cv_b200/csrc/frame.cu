@@ -105,21 +105,33 @@ int cvb_frame_features_batch_dev(cvb_ctx *ctx, const cvb_keypoint *kp_dev, const
 int cvb_frame_features_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, const uint8_t *rgb, uint32_t batch, uint32_t w,
                              uint32_t h, const cvb_intrinsics_k1 *intrinsics, cvb_keypoint *kp_out, uint8_t *desc_out, double *bearings_out,
                              uint8_t *colors_out, uint32_t cap, uint32_t *n_out) {
+    return frame_features_batch_host(ctx, cfg, images, rgb, false, batch, w, h, intrinsics, kp_out, desc_out, bearings_out, colors_out, cap,
+                                     n_out);
+}
+
+}  // extern "C"
+
+int frame_features_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, const uint8_t *rgb, bool planes_on_device,
+                              uint32_t batch, uint32_t w, uint32_t h, const cvb_intrinsics_k1 *intrinsics, cvb_keypoint *kp_out,
+                              uint8_t *desc_out, double *bearings_out, uint8_t *colors_out, uint32_t cap, uint32_t *n_out) {
     if (!ctx) return CVB_EINVAL;
     if (!cfg || !images || !rgb || !intrinsics || !n_out || (cap && (!kp_out || !desc_out || !bearings_out || !colors_out)))
         return cvb_set_error(ctx, CVB_EINVAL, "null argument");
     if (batch == 0 || w == 0 || h == 0) return cvb_set_error(ctx, CVB_EINVAL, "empty image or batch");
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t px = (size_t)batch * w * h, slots = (size_t)batch * std::max<uint32_t>(cap, 1);
-    int rc = ensure_frame(ctx, batch, px, slots);
+    int rc = ensure_frame(ctx, batch, planes_on_device ? 0 : px, slots);
     if (rc) return rc;
     FrameWorkspace *fw = ctx->frame;
     const uint32_t cd = std::max<uint32_t>(cap, 1);
     cudaStream_t st = ctx->stream;
-    CVB_CUDA(ctx, cudaMemcpyAsync(fw->img, images, sizeof(float) * px, cudaMemcpyHostToDevice, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(fw->rgb, rgb, 3 * px, cudaMemcpyHostToDevice, st));
-    if ((rc = cvb_akaze_extract_batch_dev(ctx, cfg, fw->img, batch, w, h, fw->kp, fw->desc, cd, fw->n))) return rc;
-    if ((rc = cvb_frame_features_batch_dev(ctx, fw->kp, fw->n, batch, cd, fw->rgb, w, h, intrinsics, fw->bear, fw->col))) return rc;
+    if (!planes_on_device) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(fw->img, images, sizeof(float) * px, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(fw->rgb, rgb, 3 * px, cudaMemcpyHostToDevice, st));
+        images = fw->img; rgb = fw->rgb;
+    }
+    if ((rc = cvb_akaze_extract_batch_dev(ctx, cfg, images, batch, w, h, fw->kp, fw->desc, cd, fw->n))) return rc;
+    if ((rc = cvb_frame_features_batch_dev(ctx, fw->kp, fw->n, batch, cd, rgb, w, h, intrinsics, fw->bear, fw->col))) return rc;
     // counts behind word 0 of the page-locked scratch, which cvb_akaze_dev_overflow fills with the flag (and then synchronises)
     uint32_t *hs = (uint32_t *)cvb_pinned(ctx, sizeof(uint32_t) * ((size_t)batch + 1));
     if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
@@ -140,5 +152,3 @@ int cvb_frame_features_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
-
-}  // extern "C"

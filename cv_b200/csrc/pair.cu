@@ -104,6 +104,16 @@ int cvb_two_view_frames_k1(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float
                            const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng, cvb_keypoint *kp_out,
                            uint8_t *desc_out, uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs, cvb_pose *model_out,
                            uint32_t *inliers_out, uint32_t *n_inliers, int32_t *found) {
+    return two_view_frames_k1_host(ctx, akaze, frames, false, w, h, better_by, intrinsics, cfg, rng, kp_out, desc_out, cap, n_out, pairs_out,
+                                   n_pairs, model_out, inliers_out, n_inliers, found);
+}
+
+}  // extern "C"
+
+int two_view_frames_k1_host(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float *frames, bool frames_on_device, uint32_t w, uint32_t h,
+                            uint32_t better_by, const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng,
+                            cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs,
+                            cvb_pose *model_out, uint32_t *inliers_out, uint32_t *n_inliers, int32_t *found) {
     if (!ctx) return CVB_EINVAL;
     if (!akaze || !frames || !intrinsics || !cfg || !rng || !kp_out || !desc_out || !n_out || !pairs_out || !n_pairs || !model_out ||
         !inliers_out || !n_inliers || !found)
@@ -111,7 +121,7 @@ int cvb_two_view_frames_k1(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float
     if (cap == 0 || w == 0 || h == 0) return cvb_set_error(ctx, CVB_EINVAL, "empty image or zero capacity");
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     const size_t px = (size_t)w * h;
-    int rc = ensure_pair(ctx, cap, 2 * px);
+    int rc = ensure_pair(ctx, cap, frames_on_device ? 0 : 2 * px);
     if (rc) return rc;
     PairWorkspace *pw = ctx->pair;
     cudaStream_t st = ctx->stream;
@@ -120,8 +130,9 @@ int cvb_two_view_frames_k1(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float
     int32_t *found_dev = (int32_t *)(n_pairs_dev + 2);
     cvb_pose *model_dev = (cvb_pose *)(pw->res + L.model);
     uint32_t *pairs_dev = (uint32_t *)(pw->res + L.pairs), *inl_dev = (uint32_t *)(pw->res + L.inliers);
-    CVB_CUDA(ctx, cudaMemcpyAsync(pw->img, frames, sizeof(float) * 2 * px, cudaMemcpyHostToDevice, st));
-    if ((rc = cvb_akaze_extract_batch_dev(ctx, akaze, pw->img, 2, w, h, pw->kp, pw->desc, pw->cap, pw->n))) return rc;
+    if (!frames_on_device) CVB_CUDA(ctx, cudaMemcpyAsync(pw->img, frames, sizeof(float) * 2 * px, cudaMemcpyHostToDevice, st));
+    if ((rc = cvb_akaze_extract_batch_dev(ctx, akaze, frames_on_device ? frames : pw->img, 2, w, h, pw->kp, pw->desc, pw->cap, pw->n)))
+        return rc;
     if ((rc = cvb_two_view_pair_k1_dev(ctx, pw->kp, pw->desc, pw->n, pw->kp + pw->cap, pw->desc + (size_t)pw->cap * 64, pw->n + 1, pw->cap,
                                        better_by, intrinsics, cfg, rng, pairs_dev, cap, n_pairs_dev, model_dev, inl_dev, n_inl_dev, found_dev)))
         return rc;
@@ -144,5 +155,3 @@ int cvb_two_view_frames_k1(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const float
     n_out[0] = hn[0]; n_out[1] = hn[1];
     return 0;
 }
-
-}  // extern "C"

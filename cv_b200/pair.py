@@ -7,6 +7,9 @@ import numpy as np
 
 from ._lib import KP_DTYPE, default_context
 from .geom import Arrsac, Pose, _lib as _geom_lib
+from .image import is_dynamic
+from .image import lib as _image_lib
+from .image import stack as _stack_frames
 from .pinhole import CameraIntrinsicsK1Distortion
 
 
@@ -66,24 +69,37 @@ class TwoViewBuffers:
 
 
 def two_view_frames(akaze, frames, camera, arrsac, better_by=24, cap=8192, buffers=None):
-    """frames: [2, H, W] float32.  akaze: cv_b200.Akaze; camera: cv_b200.CameraIntrinsics (cvb_two_view_frames) or
-    cv_b200.CameraIntrinsicsK1Distortion (cvb_two_view_frames_k1); arrsac: cv_b200.Arrsac (its generator
+    """frames: [2, H, W] float32, or two DynamicImage of one size and format (cvb_two_view_frames_dynamic_k1: uploaded as they are and
+    converted on the device; a CameraIntrinsics goes in as k1 = 0).  akaze: cv_b200.Akaze; camera: cv_b200.CameraIntrinsics
+    (cvb_two_view_frames) or cv_b200.CameraIntrinsicsK1Distortion (cvb_two_view_frames_k1); arrsac: cv_b200.Arrsac (its generator
     advances as the reference's would).  Returns dict(keypoints, descriptors, matches [[a, b], ...], pose (R, t) or None,
     inliers (indices into matches))."""
-    frames = np.ascontiguousarray(frames, np.float32)
-    if frames.ndim != 3 or frames.shape[0] != 2:
-        raise ValueError("frames must be [2, H, W] float32")
+    dynamic = is_dynamic(frames)
+    if dynamic:
+        if isinstance(frames, (list, tuple)) and len(frames) != 2:
+            raise ValueError("frames must be two DynamicImage")
+        fmt, pixels, W, H = _stack_frames(frames)
+        if pixels.shape[0] != 2:
+            raise ValueError("frames must be two DynamicImage")
+    else:
+        frames = np.ascontiguousarray(frames, np.float32)
+        if frames.ndim != 3 or frames.shape[0] != 2:
+            raise ValueError("frames must be [2, H, W] float32")
+        pixels, H, W = frames, frames.shape[1], frames.shape[2]
     ctx = akaze._ctx()
     _geom_lib(ctx)
     L = ctx.lib
     bind(L)
     b = buffers or TwoViewBuffers(cap)
     cfg = akaze.config.to_c()
-    if isinstance(camera, CameraIntrinsicsK1Distortion):
+    if dynamic:
+        K, IL = IntrinsicsK1.from_camera(camera), _image_lib()
+        entry = lambda *a: IL.cvb_two_view_frames_dynamic_k1(a[0], a[1], fmt, *a[2:])   # noqa: E731
+    elif isinstance(camera, CameraIntrinsicsK1Distortion):
         K, entry = IntrinsicsK1.from_camera(camera), L.cvb_two_view_frames_k1
     else:
         K, entry = Intrinsics.from_camera(camera), L.cvb_two_view_frames
-    ctx.check(entry(ctx.handle, C.addressof(cfg), frames.ctypes.data, frames.shape[2], frames.shape[1], better_by, C.byref(K),
+    ctx.check(entry(ctx.handle, C.addressof(cfg), pixels.ctypes.data, W, H, better_by, C.byref(K),
                     C.addressof(arrsac.cfg), C.addressof(arrsac.rng.state), b.kp.ctypes.data, b.desc.ctypes.data, b.cap,
                     b.n.ctypes.data, b.pairs.ctypes.data, C.addressof(b.n_pairs), C.addressof(b.model), b.inliers.ctypes.data,
                     C.addressof(b.n_inliers), C.addressof(b.found)))
