@@ -192,3 +192,6 @@ pub mod pinhole;
 
 // ---- INTEGRATION.md section 2g (include/cvb200_image.h) ----
 pub mod dynamic;
+
+// ---- INTEGRATION.md section 2h (include/cvb200_filter.h) ----
+pub mod filter;

@@ -4,6 +4,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
 
   Akaze                 <- akaze::Akaze                       (akaze/src/lib.rs:109-185, 295-366)
   DynamicImage          <- image::DynamicImage's integer variants, from_dynamic on the device (akaze/src/image.rs:45-109)
+  horizontal_filter, vertical_filter, separable_filter, gaussian_kernel, gaussian_blur, half_size
+                        <- akaze::image                        (akaze/src/image.rs:154-389)
   KeyPoint dtype        <- akaze::KeyPoint                    (akaze/src/lib.rs:71-93)
   LinearKnn / hamming_knn <- space::LinearKnn + bitarray::Hamming (call sites akaze/tests/estimate_pose.rs:78-97)
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
@@ -19,6 +21,7 @@ CvbError when the library or a Hopper (sm_90) GPU is missing.
 from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F401
 from .akaze import Akaze, AkazeConfig  # noqa: F401
 from .image import DynamicImage  # noqa: F401
+from .filter import gaussian_blur, gaussian_kernel, half_size, horizontal_filter, separable_filter, vertical_filter  # noqa: F401
 from .knn import HammingHasher, LinearKnn, hamming_knn, lowe_ratio_matches, matching, symmetric_matching  # noqa: F401
 from .pinhole import (CameraIntrinsics, CameraIntrinsicsK1Distortion, EssentialMatrix, average_pose_reprojection_error,  # noqa: F401
                       average_pose_reprojection_error_batch, pose_reprojection_error, pose_reprojection_error_batch)

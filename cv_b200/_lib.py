@@ -1,6 +1,6 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
-cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h) and cv_b200/libcvb200_image.so
-(include/cvb200_image.h)."""
+cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
+(include/cvb200_image.h) and cv_b200/libcvb200_filter.so (include/cvb200_filter.h)."""
 import ctypes as C
 import os
 
@@ -84,6 +84,13 @@ PINHOLE_ABI_SYMBOLS = [
 IMAGE_ABI_SYMBOLS = [
     "cvb_gray_float_from_dynamic_dev", "cvb_akaze_extract_dynamic_batch", "cvb_akaze_extract_dynamic_batch_dev",
     "cvb_frame_features_dynamic_batch", "cvb_two_view_frames_dynamic_k1",
+]
+
+# every symbol include/cvb200_filter.h declares (akaze::image: filters, Gaussian kernel and blur, half_size), exported by
+# libcvb200_filter.so; checked by tests/test_abi_filter.py
+FILTER_ABI_SYMBOLS = [
+    "cvb_gaussian_kernel", "cvb_horizontal_filter", "cvb_horizontal_filter_dev", "cvb_vertical_filter", "cvb_vertical_filter_dev",
+    "cvb_separable_filter", "cvb_separable_filter_dev", "cvb_gaussian_blur", "cvb_gaussian_blur_dev", "cvb_half_size", "cvb_half_size_dev",
 ]
 
 
@@ -195,6 +202,25 @@ def load_image_library():
             raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
         _IMAGE_LIB = C.CDLL(p)
     return _IMAGE_LIB
+
+
+_FILTER_LIB = None
+
+
+def filter_lib_path():
+    return os.path.join(_HERE, "libcvb200_filter.so")
+
+
+def load_filter_library():
+    """Loads libcvb200_filter.so, the module of include/cvb200_filter.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _FILTER_LIB
+    if _FILTER_LIB is None:
+        load_library()
+        p = filter_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        _FILTER_LIB = C.CDLL(p)
+    return _FILTER_LIB
 
 
 class Context:

@@ -64,7 +64,9 @@ std::vector<double> fed_tau_by_process_time(double T, double tau_max) {
     return out;
 }
 
-// image.rs:349-374
+}  // namespace
+
+// image.rs:349-374 (also cvb_gaussian_kernel of include/cvb200_filter.h)
 void gaussian_kernel_host(float r, int ks, float *out) {
     int half = ks / 2;
     float sum = 0.f;
@@ -78,6 +80,18 @@ void gaussian_kernel_host(float r, int ks, float *out) {
     }
     for (int i = 0; i < ks; i++) out[i] /= sum;
 }
+
+// cvb_half_size(_dev) of include/cvb200_filter.h: the extractor's kernel on packed planes
+int half_size_launch(cvb_ctx *ctx, const float *in, float *out, uint32_t batch, uint32_t w, uint32_t h) {
+    const unsigned hw = w / 2, hh = h / 2;
+    dim3 blk(32, 8), grd(cdiv(hw, 32), cdiv(hh, 8), batch);
+    CVB_PROF(ctx, "k_half_size", 4.0 * ((double)w * h + (double)hw * hh) * batch);
+    k_half_size<<<grd, blk, 0, ctx->stream>>>(in, out, (int)w, (int)h, (size_t)w * h, (size_t)hw * hh);
+    CVB_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+namespace {
 
 int make_gauss_taps(float r, Taps *t) {
     int radius = (int)ceilf(2.0f * r);   // image.rs:385

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 #include "../../include/cvb200_sfm.h"   // includes cvb200.h
@@ -12,6 +13,7 @@ struct GeomWorkspace;
 struct PairWorkspace;
 struct FrameWorkspace;
 struct ImageWorkspace;
+struct FilterWorkspace;
 
 struct cvb_ctx {
     int device = 0;
@@ -28,6 +30,7 @@ struct cvb_ctx {
     PairWorkspace *pair = nullptr;
     FrameWorkspace *frame = nullptr;
     ImageWorkspace *image = nullptr;
+    FilterWorkspace *filter = nullptr;
     // page-locked host scratch for the small device->host results of the host API (a D2H copy into pageable memory is
     // staged synchronously inside the driver and stalls the other contexts' launches)
     void *pinned = nullptr;
@@ -64,6 +67,7 @@ void geom_workspace_free(GeomWorkspace *ws);
 void pair_workspace_free(PairWorkspace *ws);
 void frame_workspace_free(FrameWorkspace *ws);
 void image_workspace_free(ImageWorkspace *ws);
+void filter_workspace_free(FilterWorkspace *ws);
 
 // Bodies of the host-API entry points cvb_akaze_extract_batch, cvb_frame_features_batch and cvb_two_view_frames_k1.  With the
 // *_on_device flag set, the f32 planes (and the RGB8 plane) are already on the device and nothing is uploaded: the pixel-format entry
@@ -77,6 +81,22 @@ int two_view_frames_k1_host(cvb_ctx *ctx, const cvb_akaze_cfg *akaze, const floa
                             uint32_t better_by, const cvb_intrinsics_k1 *intrinsics, const cvb_arrsac_cfg *cfg, cvb_rng *rng,
                             cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out, uint32_t *pairs_out, uint32_t *n_pairs,
                             cvb_pose *model_out, uint32_t *inliers_out, uint32_t *n_inliers, int32_t *found);
+
+// akaze.cu pieces the public image module (filter.cu, include/cvb200_filter.h) reuses: gaussian_kernel (image.rs:349-374) on the host, and
+// one launch of the extractor's k_half_size over `batch` packed planes (out: batch planes of (w / 2) x (h / 2), both non-empty).
+void gaussian_kernel_host(float r, int ks, float *out);
+int half_size_launch(cvb_ctx *ctx, const float *in, float *out, uint32_t batch, uint32_t w, uint32_t h);
+
+// A device buffer of the context's workspaces grown to >= n elements (contents not kept); waits for the stream before freeing.
+template <typename T>
+int ws_grow(cvb_ctx *ctx, T **p, size_t *have, size_t n) {
+    if (*have >= n) return 0;
+    if (*p) { cvb_wait(ctx, ctx->stream); cudaFree(*p); *p = nullptr; *have = 0; }
+    const cudaError_t e = cudaMalloc((void **)p, std::max<size_t>(n, 1) * sizeof(T));
+    if (e != cudaSuccess) return cvb_set_error(ctx, CVB_ENOMEM, "cudaMalloc: %s", cudaGetErrorString(e));
+    *have = n;
+    return 0;
+}
 
 #define CVB_CUDA(ctx, call)                                                                          \
     do {                                                                                             \

@@ -118,6 +118,7 @@ void cvb_ctx_destroy(cvb_ctx *ctx) {
     pair_workspace_free(ctx->pair);
     frame_workspace_free(ctx->frame);
     image_workspace_free(ctx->image);
+    filter_workspace_free(ctx->filter);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev_wait) cudaEventDestroy(ctx->ev_wait);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);

@@ -111,16 +111,6 @@ int check_format(cvb_ctx *ctx, cvb_pixel_format format, bool rgb, uint32_t batch
     return 0;
 }
 
-template <typename T>
-int grow(cvb_ctx *ctx, T **p, size_t *have, size_t n) {
-    if (*have >= n) return 0;
-    if (*p) { cvb_wait(ctx, ctx->stream); cudaFree(*p); *p = nullptr; *have = 0; }
-    const cudaError_t e = cudaMalloc((void **)p, std::max<size_t>(n, 1) * sizeof(T));
-    if (e != cudaSuccess) return cvb_set_error(ctx, CVB_ENOMEM, "cudaMalloc: %s", cudaGetErrorString(e));
-    *have = n;
-    return 0;
-}
-
 ImageWorkspace *workspace(cvb_ctx *ctx) {
     if (!ctx->image) ctx->image = new ImageWorkspace();
     return ctx->image;
@@ -158,8 +148,8 @@ int upload_and_convert(cvb_ctx *ctx, cvb_pixel_format format, const void *pixels
     const size_t npx = (size_t)batch * w * h, bytes = npx * bytes_per_pixel(format);
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
     int rc;
-    if ((rc = grow(ctx, &iw->raw, &iw->raw_bytes, bytes)) || (rc = grow(ctx, &iw->gray, &iw->gray_px, npx))) return rc;
-    if (rgb && (rc = grow(ctx, &iw->rgb, &iw->rgb_px, 3 * npx))) return rc;
+    if ((rc = ws_grow(ctx, &iw->raw, &iw->raw_bytes, bytes)) || (rc = ws_grow(ctx, &iw->gray, &iw->gray_px, npx))) return rc;
+    if (rgb && (rc = ws_grow(ctx, &iw->rgb, &iw->rgb_px, 3 * npx))) return rc;
     CVB_CUDA(ctx, cudaMemcpyAsync(iw->raw, pixels, bytes, cudaMemcpyHostToDevice, ctx->stream));
     return launch_from_dynamic(ctx, format, iw->raw, npx, iw->gray, rgb ? iw->rgb : nullptr);
 }
@@ -197,7 +187,7 @@ int img_akaze_extract_dynamic_batch_dev(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, 
     ImageWorkspace *iw = workspace(ctx);
     const size_t npx = (size_t)batch * w * h;
     CVB_CUDA(ctx, cudaSetDevice(ctx->device));
-    if ((rc = grow(ctx, &iw->gray, &iw->gray_px, npx))) return rc;
+    if ((rc = ws_grow(ctx, &iw->gray, &iw->gray_px, npx))) return rc;
     if ((rc = launch_from_dynamic(ctx, format, pixels_dev, npx, iw->gray, nullptr))) return rc;
     return cvb_akaze_extract_batch_dev(ctx, cfg, iw->gray, batch, w, h, kp_out_dev, desc_out_dev, cap, n_out_dev);
 }
