@@ -195,3 +195,6 @@ pub mod dynamic;
 
 // ---- INTEGRATION.md section 2h (include/cvb200_filter.h) ----
 pub mod filter;
+
+// ---- INTEGRATION.md section 2i (include/cvb200_lsh.h) ----
+pub mod lsh;

@@ -8,6 +8,7 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
                         <- akaze::image                        (akaze/src/image.rs:154-389)
   KeyPoint dtype        <- akaze::KeyPoint                    (akaze/src/lib.rs:71-93)
   LinearKnn / hamming_knn <- space::LinearKnn + bitarray::Hamming (call sites akaze/tests/estimate_pose.rs:78-97)
+  hash_knn / FrameHashIndex <- cv-sfm's similar-frame search, lsh_to_frame.knn_values (cv-sfm/src/lib.rs:597-668), exact
   matching / symmetric_matching <- cv-sfm/src/lib.rs:3097-3133, tutorial-code chapter4 main.rs:91-137
   CameraIntrinsics(K1Distortion) <- cv-pinhole/src/lib.rs:32-240
   *pose_reprojection_error, EssentialMatrix <- cv-pinhole/src/lib.rs:314-372, essential.rs:56-275
@@ -22,7 +23,8 @@ from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F
 from .akaze import Akaze, AkazeConfig  # noqa: F401
 from .image import DynamicImage  # noqa: F401
 from .filter import gaussian_blur, gaussian_kernel, half_size, horizontal_filter, separable_filter, vertical_filter  # noqa: F401
-from .knn import HammingHasher, LinearKnn, hamming_knn, lowe_ratio_matches, matching, symmetric_matching  # noqa: F401
+from .knn import (FrameHashIndex, HammingHasher, LinearKnn, hash_knn, hamming_knn, lowe_ratio_matches, matching,  # noqa: F401
+                  symmetric_matching)
 from .pinhole import (CameraIntrinsics, CameraIntrinsicsK1Distortion, EssentialMatrix, average_pose_reprojection_error,  # noqa: F401
                       average_pose_reprojection_error_batch, pose_reprojection_error, pose_reprojection_error_batch)
 from .geom import (Arrsac, EightPoint, LambdaTwist, NisterStewenius, Pcg64, Xoshiro256PlusPlus,  # noqa: F401

@@ -1,6 +1,6 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
-(include/cvb200_image.h) and cv_b200/libcvb200_filter.so (include/cvb200_filter.h)."""
+(include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h) and cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h)."""
 import ctypes as C
 import os
 
@@ -91,6 +91,12 @@ IMAGE_ABI_SYMBOLS = [
 FILTER_ABI_SYMBOLS = [
     "cvb_gaussian_kernel", "cvb_horizontal_filter", "cvb_horizontal_filter_dev", "cvb_vertical_filter", "cvb_vertical_filter_dev",
     "cvb_separable_filter", "cvb_separable_filter_dev", "cvb_gaussian_blur", "cvb_gaussian_blur_dev", "cvb_half_size", "cvb_half_size_dev",
+]
+
+# every symbol include/cvb200_lsh.h declares (exact Hamming k-NN over frame hashes: cv-sfm's similar-frame search), exported by
+# libcvb200_lsh.so; checked by tests/test_abi_lsh.py
+LSH_ABI_SYMBOLS = [
+    "cvb_hash_knn", "cvb_hash_knn_dev",
 ]
 
 
@@ -221,6 +227,25 @@ def load_filter_library():
             raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
         _FILTER_LIB = C.CDLL(p)
     return _FILTER_LIB
+
+
+_LSH_LIB = None
+
+
+def lsh_lib_path():
+    return os.path.join(_HERE, "libcvb200_lsh.so")
+
+
+def load_lsh_library():
+    """Loads libcvb200_lsh.so, the module of include/cvb200_lsh.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _LSH_LIB
+    if _LSH_LIB is None:
+        load_library()
+        p = lsh_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        _LSH_LIB = C.CDLL(p)
+    return _LSH_LIB
 
 
 class Context:

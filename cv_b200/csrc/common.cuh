@@ -14,6 +14,7 @@ struct PairWorkspace;
 struct FrameWorkspace;
 struct ImageWorkspace;
 struct FilterWorkspace;
+struct LshWorkspace;
 
 struct cvb_ctx {
     int device = 0;
@@ -31,6 +32,7 @@ struct cvb_ctx {
     FrameWorkspace *frame = nullptr;
     ImageWorkspace *image = nullptr;
     FilterWorkspace *filter = nullptr;
+    LshWorkspace *lsh = nullptr;
     // page-locked host scratch for the small device->host results of the host API (a D2H copy into pageable memory is
     // staged synchronously inside the driver and stalls the other contexts' launches)
     void *pinned = nullptr;
@@ -68,6 +70,7 @@ void pair_workspace_free(PairWorkspace *ws);
 void frame_workspace_free(FrameWorkspace *ws);
 void image_workspace_free(ImageWorkspace *ws);
 void filter_workspace_free(FilterWorkspace *ws);
+void lsh_workspace_free(LshWorkspace *ws);
 
 // Bodies of the host-API entry points cvb_akaze_extract_batch, cvb_frame_features_batch and cvb_two_view_frames_k1.  With the
 // *_on_device flag set, the f32 planes (and the RGB8 plane) are already on the device and nothing is uploaded: the pixel-format entry

@@ -119,6 +119,7 @@ void cvb_ctx_destroy(cvb_ctx *ctx) {
     frame_workspace_free(ctx->frame);
     image_workspace_free(ctx->image);
     filter_workspace_free(ctx->filter);
+    lsh_workspace_free(ctx->lsh);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev_wait) cudaEventDestroy(ctx->ev_wait);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
