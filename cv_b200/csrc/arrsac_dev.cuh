@@ -49,6 +49,10 @@ struct ArrsacCtl {
     uint32_t stat_walk_us, stat_commit_us;   // SPRT: time in the chunk walks / in the commit turns (globaltimer)
     uint32_t stat_perm_us, stat_turns;       // SPRT: time in the ordering step in front of the walks; commit turns in total
     uint32_t q_blk, stat_qblk;               // undecided predicates queued by the current block's scoring (queue region 0); over all blocks
+    uint32_t stat_units_kept, stat_units_new; // block loop: 32-datum units of kept rows / of new models (valid poses)
+    uint32_t stat_skip;                      // new-model units written 0 by early rejection instead of scored
+    uint32_t stat_blk_w0, stat_blk_lt32;     // blocks with new models scored under worst == 0 / under acc_hi - worst < 32
+    uint32_t stat_blk_bar0;                  // blocks whose new samples were drawn but not estimated (worst >= acc_hi)
 };
 
 struct ArrsacParams {            // launch-constant configuration (by value)
@@ -60,6 +64,7 @@ struct ArrsacParams {            // launch-constant configuration (by value)
     uint32_t rows;               // candidate rows per table (max_cand + G * MM)
     uint32_t prefix, cmin;       // initial scoring in two stages: all words for the first `prefix` samples; for the rest, words >= 1 only
                                  // when the first 32 data hold >= cmin inliers (the SPRT computes a missing word itself if it ever needs one)
+    uint32_t early;              // block scoring stops scoring new models that can no longer beat the bar (k_ars_score phase 1)
     float lr_thr, eps0, delta0;
     double thr;
     int row0;
@@ -299,17 +304,18 @@ __device__ __forceinline__ bool ars_inlier(const cvb_pose &Pz, const double *__r
 
 // the scoring kernels' predicate: the exact evaluation costs ~8x the filter, so an undecided pair goes to a queue that a resolve
 // kernel works off without divergence (one undecided lane would otherwise stall its warp for the whole Jacobi iteration) and
-// counts as an outlier until then; `src` tells the resolve kernel which pose and mask row the entry belongs to
+// counts as an outlier until then; `src` tells the resolve kernel which pose and mask row the entry belongs to.
+// Returns 1 (inlier), 0 (certain outlier) or -1 (queued: its mask bit is 0 until k_ars_resolve* decides it).
 template <int RES>
-__device__ __forceinline__ bool ars_inlier_queued(const cvb_pose &Pz, const double *__restrict__ a, const double *__restrict__ b, uint32_t i,
-                                                  double thr, uint32_t *qc, uint2 *q, uint32_t src) {
-    if (RES == 1) return ars_inlier<RES>(Pz, a, b, i, thr);
+__device__ __forceinline__ int ars_inlier_queued(const cvb_pose &Pz, const double *__restrict__ a, const double *__restrict__ b, uint32_t i,
+                                                 double thr, uint32_t *qc, uint2 *q, uint32_t src) {
+    if (RES == 1) return ars_inlier<RES>(Pz, a, b, i, thr) ? 1 : 0;
     const double *pa = a + 3 * (size_t)i, *pb = b + 3 * (size_t)i;
     const int f = c2c_inlier_filter(Pz.r, Pz.t, pa, pb, thr);
-    if (f >= 0) return f != 0;
+    if (f >= 0) return f != 0 ? 1 : 0;
     const uint32_t slot = atomicAdd(qc, 1u);
-    if (slot < ARS_QCAP) { q[slot] = make_uint2(src, i); return false; }
-    return ars_exact_c2c(&Pz, pa, pb, thr);
+    if (slot < ARS_QCAP) { q[slot] = make_uint2(src, i); return -1; }
+    return ars_exact_c2c(&Pz, pa, pb, thr) ? 1 : 0;
 }
 
 // are the mask words >= 1 of an initial model computed by the scoring kernels?  (word0 = its final first mask word)
@@ -321,13 +327,14 @@ __device__ __forceinline__ bool ars_ready(uint32_t word0, uint32_t init_n, uint3
 
 // phase 0 / 2: the initial models on data [0, init_n) -> masks0[model * W0 + w] (two stages, see ArrsacParams::prefix)
 // phase 1: kept candidate rows on [blk_lo, blk_hi) merged into their mask rows; new models on [0, blk_hi) -> newmask rows
+//          (nout[j]: certain outliers of new model j in [0, acc_hi) so far; zero on entry, k_ars_book clears it for the next block)
 template <int RES>
 __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__restrict__ queue, ArrsacParams P, int phase, const double *__restrict__ a,
                                                    const double *__restrict__ b, const cvb_pose *__restrict__ poses0,
                                                    const uint8_t *__restrict__ nposes0, uint32_t *__restrict__ masks0,
                                                    const cvb_pose *__restrict__ tposes, uint32_t *__restrict__ tmasks,
                                                    const cvb_pose *__restrict__ newposes, const uint8_t *__restrict__ nposes_new,
-                                                   uint32_t *__restrict__ newmask) {
+                                                   uint32_t *__restrict__ newmask, uint32_t *nout) {
     if (ctl->done) return;
     const unsigned full = 0xffffffffu;
     const uint32_t lane = threadIdx.x & 31;
@@ -350,41 +357,72 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
             if (phase == 2 && !ars_ready(masks0[(size_t)m * P.W0], init_n, m / P.MM, P)) continue;
             const uint32_t i = w * 32 + lane;
             bool bit = false;
-            if (i < init_n) bit = ars_inlier_queued<RES>(poses0[m], a, b, i, P.thr, qc, q, m);      // queue: k_ars_resolve
+            if (i < init_n) bit = ars_inlier_queued<RES>(poses0[m], a, b, i, P.thr, qc, q, m) > 0;      // queue: k_ars_resolve
             const unsigned bits = __ballot_sync(full, bit);
             if (lane == 0) { masks0[(size_t)m * P.W0 + w] = bits; atomicAdd(phase == 0 ? &ctl->stat_units0 : &ctl->stat_units2, 1u); }
         }
         return;
     }
     const uint32_t lo = ctl->blk_lo, hi = ctl->blk_hi, Hn = ctl->Hn, cur = ctl->cur;
+    const uint32_t worst = ctl->worst;
     const uint32_t wlo = lo >> 5, nwb = hi > lo ? ((hi - 1) >> 5) - wlo + 1 : 0;
     const uint32_t kept_units = Hn * nwb;
     const uint32_t nnew = ctl->n_new * P.MM, nwn = (hi + 31) >> 5;
     const uint32_t units = kept_units + nnew * nwn;
     const cvb_pose *tp = tposes + (size_t)cur * P.rows;
     uint32_t *tm = tmasks + (size_t)cur * P.rows * P.NW;
+    // Early rejection of new models.  k_ars_book accepts new model j only when its mask holds more than `worst` inliers in
+    // [0, acc_hi); both values were written by the previous k_ars_book, which sets acc_hi = blk_lo (so does k_ars_sprt).  Once
+    // bar = acc_hi - worst data of that range are CERTAIN outliers of j (filter result 0, counted in nout[j]; queued predicates are
+    // not counted), j has at most `worst` inliers there and will be rejected, so its remaining mask words are written 0 instead of
+    // scored.  The result stays exact:
+    // k_ars_resolve_block only ORs real inliers into a word, so the popcount k_ars_book takes of j stays <= its true count <= worst
+    // and j is rejected by the same test as with every word scored; the mask of a rejected model is never read again.  (bar = 0,
+    // worst >= acc_hi: no new model can beat the bar, and k_ars_book leaves such a block without new models.)  New-model units run word-major -- word w of every model, then word w + 1 --
+    // so that a model's early words are decided before its later ones start.  Kept rows are scored in full.
+    const uint32_t bar = lo > worst ? lo - worst : 0;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {           // CVB_ARS_DEBUG counters
+        uint32_t valid = 0;
+        for (uint32_t s = 0; s < ctl->n_new; s++) valid += min((uint32_t)nposes_new[s], P.MM);
+        ctl->stat_units_kept += kept_units; ctl->stat_units_new += valid * nwn;
+        if (nnew) { ctl->stat_blk_w0 += worst == 0; ctl->stat_blk_lt32 += bar < 32; }
+    }
+    uint32_t skipped = 0;                                // units this warp wrote 0 instead of scoring
     // undecided predicates go to queue region 0 (free once the initial stages are resolved) for k_ars_resolve_block:
     // entry source r < P.rows is kept row r, P.rows + j is new model j
     for (uint32_t u = warp; u < units; u += nwarps) {
-        if (u < kept_units) {
-            const uint32_t r = u / nwb, w = wlo + u % nwb;
-            const uint32_t i = w * 32 + lane;
-            const bool act = i >= lo && i < hi;
-            bool bit = false;
-            if (act) bit = ars_inlier_queued<RES>(tp[r], a, b, i, P.thr, &ctl->q_blk, queue, r);
-            const unsigned bits = __ballot_sync(full, bit), range = __ballot_sync(full, act);
-            if (lane == 0) { uint32_t *p = tm + (size_t)r * P.NW + w; *p = (*p & ~range) | bits; }
-        } else {
-            const uint32_t v = u - kept_units;
-            const uint32_t j = v / nwn, w = v % nwn;
+        // one predicate site for both kinds of unit (two inlined copies of the filter cost registers)
+        const bool kept = u < kept_units;
+        uint32_t src, w;                                 // src: queue source (kept row r, or P.rows + new model j)
+        if (kept) { src = u / nwb; w = wlo + u % nwb; }
+        else {
+            const uint32_t v = u - kept_units, j = v % nnew;
             if ((j % P.MM) >= nposes_new[j / P.MM]) continue;
-            const uint32_t i = w * 32 + lane;
-            bool bit = false;
-            if (i < hi) bit = ars_inlier_queued<RES>(newposes[j], a, b, i, P.thr, &ctl->q_blk, queue, P.rows + j);
-            const unsigned bits = __ballot_sync(full, bit);
-            if (lane == 0) newmask[(size_t)j * P.NW + w] = bits;
+            src = P.rows + j; w = v / nnew;
+            if (P.early && __ldcg(nout + j) >= bar) {          // the same address in every lane: the branch is warp-uniform
+                if (lane == 0) newmask[(size_t)j * P.NW + w] = 0u;
+                skipped++;
+                continue;
+            }
+        }
+        const uint32_t i = w * 32 + lane;
+        const bool act = i < hi && (!kept || i >= lo);
+        int f = -1;
+        if (act) f = ars_inlier_queued<RES>(kept ? tp[src] : newposes[src - P.rows], a, b, i, P.thr, &ctl->q_blk, queue, src);
+        const unsigned bits = __ballot_sync(full, f > 0);
+        if (kept) {
+            const unsigned range = __ballot_sync(full, act);
+            if (lane == 0) { uint32_t *p = tm + (size_t)src * P.NW + w; *p = (*p & ~range) | bits; }
+        } else {
+            const uint32_t j = src - P.rows;
+            const unsigned out = __ballot_sync(full, f == 0 && i < lo);
+            if (lane == 0) {
+                newmask[(size_t)j * P.NW + w] = bits;
+                if (P.early && out) atomicAdd(nout + j, (uint32_t)__popc(out));
+            }
         }
     }
+    if (lane == 0 && skipped) atomicAdd(&ctl->stat_skip, skipped);
 }
 
 // exact evaluation of the queued predicates of the initial scoring; inliers are OR-ed into their mask word
@@ -876,7 +914,8 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_book(ArrsacCtl *ctl, Arrsac
                                                            cvb_pose *tposes, uint32_t *tinl, uint32_t *tmasks,
                                                            const cvb_pose *__restrict__ newposes, const uint8_t *__restrict__ nposes_new,
                                                            const uint32_t *__restrict__ newmask, uint32_t *__restrict__ pool,
-                                                           uint32_t *__restrict__ samples_new, unsigned long long loop_cond) {
+                                                           uint32_t *__restrict__ samples_new, uint32_t *__restrict__ nout,
+                                                           unsigned long long loop_cond) {
     // loop_cond: the handle of the graph's WHILE node when the block loop is a device-side loop (0 = unrolled launches);
     // the node re-runs its body while the value is non-zero, so the loop's end is the one thing this kernel has to report
     if (ctl->done) { if (loop_cond && threadIdx.x == 0) cudaGraphSetConditional(loop_cond, 0); return; }
@@ -987,10 +1026,16 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_book(ArrsacCtl *ctl, Arrsac
     }
     const bool gen = npool >= P.K && P.G > 0;
     if (gen) ars_sample_block(ctl, raw, npool, P.K, P.G, samples_new, pool, (uint32_t *)keys /* free: the keys were consumed above */, sm + 64);
+    for (uint32_t j = tid; j < P.G * P.MM; j += NT) nout[j] = 0;     // the next block's scoring counts its new models' outliers from 0
     __syncthreads();
     if (tid == 0) {
+        // A new hypothesis joins the candidates only with more than worst_next inliers in [0, hi).  When worst_next >= hi none can,
+        // whatever its pose: its sample is still drawn above (the generator advances exactly as in the reference), but it is neither
+        // estimated nor scored.
+        const bool bar0 = worst_next >= hi;
         ctl->worst = worst_next;
-        ctl->n_new = gen ? P.G : 0;
+        ctl->n_new = gen && !bar0 ? P.G : 0;
+        ctl->stat_blk_bar0 += gen && bar0;
         ctl->cur = cur ^ 1; ctl->Hn = keep;
         ctl->acc_hi = hi; ctl->blk_lo = hi; ctl->blk_hi = min(hi + P.bs, n);
         ctl->iters++;

@@ -1629,7 +1629,7 @@ struct DevBuf {
 // device-resident ARRSAC (arrsac_dev.cuh): buffers + page-locked staging of one context
 struct ArsWorkspace {
     DevBuf ctl, raw, samples0, poses0, nposes0, masks0, vm, pass_id, pass_inl, tposes, tinl, tmasks, newposes, nposes_new, newmask,
-        pool, samples_new, res, queue;
+        nout, pool, samples_new, res, queue;
     uint32_t *h_raw = nullptr;      // page-locked: raw draws + ArrsacCtl header
     size_t h_raw_cap = 0;
     unsigned char *h_res = nullptr; // page-locked result block
@@ -1642,7 +1642,7 @@ struct ArsWorkspace {
     // depends on; a key is captured the second time it is seen (a one-off call does not pay the instantiation)
     struct GraphKey {
         ArrsacParams P; int kind, row0; const void *a, *b, *n_dev; uint32_t n_host, nmax, cap, nb; const void *model, *inl, *ninl, *found;
-        const void *ws[21];
+        const void *ws[22];
     };
     struct GraphEntry { GraphKey key; cudaGraphExec_t exec; uint64_t launches; uint32_t body; };   // body: launches of one WHILE body (0: no WHILE node)
     uint32_t last_body = 0;         // the pending run went through a WHILE-node graph with this many launches per body (counted at commit)
@@ -1932,6 +1932,8 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     { const char *env = getenv("CVB_ARS_EAGER"); const bool eager = (env && env[0] == '1') || kind_res(kind) == 1;
       P.prefix = eager ? P.H0 : std::min<uint32_t>(P.H0, 64); P.cmin = 2;
       if (const char *cm = getenv("CVB_ARS_CMIN")) P.cmin = (uint32_t)std::max(0, atoi(cm)); }
+    // early rejection in the block scoring (arrsac_dev.cuh, k_ars_score phase 1); CVB_ARS_EARLY_REJECT=0 scores every word
+    { const char *e = getenv("CVB_ARS_EARLY_REJECT"); P.early = (e && e[0] == '0') ? 0u : 1u; }
     if (P.max_cand == 0 || P.rows > ARS_SORT_CAP)
         return cvb_set_error(ctx, CVB_EUNSUPPORTED, "max_candidate_hypotheses + estimations_per_block * %u must be in 1..%u", P.MM, ARS_SORT_CAP);
     if ((uint64_t)P.bs * P.ib + 1 > 2ull * ARS_SORT_CAP) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "block_size * initialization_blocks too large");
@@ -1956,6 +1958,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     if ((rc = w->newposes.ensure(ctx, sizeof(cvb_pose) * nnew))) return rc;
     if ((rc = w->nposes_new.ensure(ctx, std::max<uint32_t>(P.G, 1)))) return rc;
     if ((rc = w->newmask.ensure(ctx, sizeof(uint32_t) * nnew * P.NW))) return rc;
+    if ((rc = w->nout.ensure(ctx, sizeof(uint32_t) * nnew))) return rc;
     if ((rc = w->pool.ensure(ctx, sizeof(uint32_t) * (size_t)P.NMAX))) return rc;
     if ((rc = w->samples_new.ensure(ctx, sizeof(uint32_t) * (size_t)std::max<uint32_t>(P.G, 1) * P.K))) return rc;
     if ((rc = w->queue.ensure(ctx, sizeof(uint2) * 2 * (size_t)ARS_QCAP))) return rc;
@@ -2024,7 +2027,9 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         };
         // the initial scoring fills the machine (4 CTAs per SM).  A block scores ~200 k predicates on 48 CTAs: a larger grid
     // lowers ONE context's latency, but with 16 pipelined contexts the small grid costs the least SM time (more units per warp, the
-    // exact-fallback stragglers amortised), and the step is bound by SM time, not by a pair's latency (not re-tuned on H100).
+    // exact-fallback stragglers amortised), and the step is bound by SM time, not by a pair's latency.  Re-tuned on one H100 80GB
+    // HBM3 (700 W) with early rejection in the block scoring: 24 / 32 / 48 / 66 / 132 CTAs gave 1 585 / 1 559-1 598 / 1 583-1 597 /
+    // 1 540-1 590 / 1 582-1 589 frames/s in the pipelined bench (two runs each), all inside the run-to-run spread, so 48 stays.
     // CVB_ARS_SGRID overrides.
     const uint32_t sgrid_full = (uint32_t)ctx->num_sms * 4;
         uint32_t sgrid_block = 48;
@@ -2040,11 +2045,13 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             if (res == 0)
                 k_ars_score<0><<<sgrid, 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
                                                       (uint32_t *)w->masks0.p, (const cvb_pose *)w->tposes.p, (uint32_t *)w->tmasks.p,
-                                                      (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p);
+                                                      (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p,
+                                                      (uint32_t *)w->nout.p);
             else
                 k_ars_score<1><<<sgrid, 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
                                                       (uint32_t *)w->masks0.p, (const cvb_pose *)w->tposes.p, (uint32_t *)w->tmasks.p,
-                                                      (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p);
+                                                      (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p,
+                                                      (uint32_t *)w->nout.p);
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
@@ -2082,7 +2089,8 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_PROF(ctx, "k_ars_book", 0);
             k_ars_book<<<1, ARS_BOOK_NT, ARS_BOOK_SMEM, st>>>(ctl, P, raw, (cvb_pose *)w->tposes.p, (uint32_t *)w->tinl.p, (uint32_t *)w->tmasks.p,
                                                               (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p,
-                                                              (const uint32_t *)w->newmask.p, (uint32_t *)w->pool.p, (uint32_t *)w->samples_new.p, cond);
+                                                              (const uint32_t *)w->newmask.p, (uint32_t *)w->pool.p, (uint32_t *)w->samples_new.p,
+                                                              (uint32_t *)w->nout.p, cond);
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
@@ -2157,7 +2165,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     key.model = model_dev; key.inl = inl_dev; key.ninl = ninl_dev; key.found = found_dev;
     {
         const DevBuf *bufs[] = {&w->ctl, &w->raw, &w->samples0, &w->poses0, &w->nposes0, &w->masks0, &w->vm, &w->pass_id, &w->pass_inl, &w->tposes,
-                                &w->tinl, &w->tmasks, &w->newposes, &w->nposes_new, &w->newmask, &w->pool, &w->samples_new, &w->queue};
+                                &w->tinl, &w->tmasks, &w->newposes, &w->nposes_new, &w->newmask, &w->nout, &w->pool, &w->samples_new, &w->queue};
         int i = 0;
         for (const DevBuf *d : bufs) key.ws[i++] = d->p;
         key.ws[i++] = w->h_raw; key.ws[i++] = w->h_res; key.ws[i++] = (const void *)(uintptr_t)nraw;
@@ -2235,8 +2243,10 @@ int arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, ArrsacCtl *stats_out = nullptr
     if (stats_out) *stats_out = *h;
     if (getenv("CVB_ARS_DEBUG"))
         fprintf(stderr, "[arrsac] n %u models %u pass %u chunks %u turns %u repairs %u lazy %u | sprt us: order %u walk %u commit %u | block iterations %u"
-                " | undecided predicates queued: initial %u block %u\n", h->n, h->Mv, h->npass, h->stat_chunks, h->stat_turns, h->stat_repairs,
-                h->stat_lazy, h->stat_perm_us, h->stat_walk_us, h->stat_commit_us, h->iters, h->q_count + h->q_count2, h->stat_qblk);
+                " | undecided predicates queued: initial %u block %u | block units: kept %u new %u skipped %u | blocks worst0 %u bar<32 %u not estimated %u\n",
+                h->n, h->Mv, h->npass, h->stat_chunks, h->stat_turns, h->stat_repairs, h->stat_lazy, h->stat_perm_us, h->stat_walk_us,
+                h->stat_commit_us, h->iters, h->q_count + h->q_count2, h->stat_qblk, h->stat_units_kept, h->stat_units_new, h->stat_skip,
+                h->stat_blk_w0, h->stat_blk_lt32, h->stat_blk_bar0);
     ctx->launches += (uint64_t)w->last_body * h->iters;          // the WHILE body ran iters + 1 times, the capture counted it once
     w->last_body = 0;
     w->pending = false;
