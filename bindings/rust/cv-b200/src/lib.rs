@@ -198,3 +198,6 @@ pub mod filter;
 
 // ---- INTEGRATION.md section 2i (include/cvb200_lsh.h) ----
 pub mod lsh;
+
+// ---- INTEGRATION.md section 2j (include/cvb200_stages.h) ----
+pub mod stages;

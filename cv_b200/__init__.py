@@ -3,6 +3,9 @@
 Host-side mirror of the reference's interfaces for this path, over the C ABI in include/cvb200.h:
 
   Akaze                 <- akaze::Akaze                       (akaze/src/lib.rs:109-185, 295-366)
+  Akaze.create_scale_space / find_image_keypoints / extract_descriptors, ScaleSpace
+                        <- akaze's staged surface: evolutions, Akaze::find_image_keypoints, Akaze::extract_descriptors
+                                                              (akaze/src/lib.rs:268-276, descriptors.rs:16-45)
   DynamicImage          <- image::DynamicImage's integer variants, from_dynamic on the device (akaze/src/image.rs:45-109)
   horizontal_filter, vertical_filter, separable_filter, gaussian_kernel, gaussian_blur, half_size
                         <- akaze::image                        (akaze/src/image.rs:154-389)
@@ -20,7 +23,7 @@ There is no CPU fallback: every call runs CUDA kernels from cv_b200/libcvb200.so
 CvbError when the library or a Hopper (sm_90) GPU is missing.
 """
 from ._lib import CvbError, Context, KP_DTYPE, lib_path, load_library  # noqa: F401
-from .akaze import Akaze, AkazeConfig  # noqa: F401
+from .akaze import Akaze, AkazeConfig, ScaleSpace  # noqa: F401
 from .image import DynamicImage  # noqa: F401
 from .filter import gaussian_blur, gaussian_kernel, half_size, horizontal_filter, separable_filter, vertical_filter  # noqa: F401
 from .knn import (FrameHashIndex, HammingHasher, LinearKnn, hash_knn, hamming_knn, lowe_ratio_matches, matching,  # noqa: F401

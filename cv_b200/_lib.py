@@ -1,6 +1,7 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
-(include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h) and cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h)."""
+(include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h) and
+cv_b200/libcvb200_stages.so (include/cvb200_stages.h)."""
 import ctypes as C
 import os
 
@@ -98,6 +99,17 @@ FILTER_ABI_SYMBOLS = [
 LSH_ABI_SYMBOLS = [
     "cvb_hash_knn", "cvb_hash_knn_dev",
 ]
+
+# every symbol include/cvb200_stages.h declares (AKAZE's staged surface: scale space, find_image_keypoints, extract_descriptors),
+# exported by libcvb200_stages.so; checked by tests/test_abi_stages.py
+STAGES_ABI_SYMBOLS = [
+    "cvb_akaze_scale_space", "cvb_akaze_scale_space_dev", "cvb_akaze_evolutions", "cvb_akaze_find_image_keypoints",
+    "cvb_akaze_find_image_keypoints_dev", "cvb_akaze_extract_descriptors", "cvb_akaze_extract_descriptors_dev",
+]
+
+# cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
+EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
+                            ("width", "<u4"), ("height", "<u4"), ("n_fed_steps", "<u4")])
 
 
 def lib_path():
@@ -246,6 +258,34 @@ def load_lsh_library():
             raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
         _LSH_LIB = C.CDLL(p)
     return _LSH_LIB
+
+
+_STAGES_LIB = None
+
+
+def stages_lib_path():
+    return os.path.join(_HERE, "libcvb200_stages.so")
+
+
+def load_stages_library():
+    """Loads libcvb200_stages.so, the module of include/cvb200_stages.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _STAGES_LIB
+    if _STAGES_LIB is None:
+        load_library()
+        p = stages_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
+        L.cvb_akaze_scale_space.argtypes = [vp, C.POINTER(AkazeCfg), vp, u32, u32, u32, C.POINTER(u64)]
+        L.cvb_akaze_scale_space_dev.argtypes = [vp, C.POINTER(AkazeCfg), vp, u32, u32, u32, C.POINTER(u64)]
+        L.cvb_akaze_evolutions.argtypes = [vp, u64, vp, u32, C.POINTER(u32)]
+        L.cvb_akaze_find_image_keypoints.argtypes = [vp, u64, vp, u32, vp]
+        L.cvb_akaze_find_image_keypoints_dev.argtypes = [vp, u64, vp, u32, vp]
+        L.cvb_akaze_extract_descriptors.argtypes = [vp, C.POINTER(AkazeCfg), u64, vp, vp, vp, vp, vp]
+        L.cvb_akaze_extract_descriptors_dev.argtypes = [vp, C.POINTER(AkazeCfg), u64, vp, vp, u32, vp, vp, vp]
+        _STAGES_LIB = L
+    return _STAGES_LIB
 
 
 class Context:

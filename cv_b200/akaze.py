@@ -1,10 +1,10 @@
 """Host-side mirror of akaze::Akaze (akaze/src/lib.rs:109-185, 295-366) over the C ABI."""
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import asdict, dataclass, replace
 
 import numpy as np
 
-from ._lib import KP_DTYPE, AkazeCfg, Context, CvbError, default_context
+from ._lib import CVB_ECAP, EVOLUTION_DTYPE, KP_DTYPE, AkazeCfg, Context, CvbError, default_context, load_stages_library
 from .image import DynamicImage, is_dynamic
 from .image import lib as _image_lib
 from .image import stack as _stack_frames
@@ -117,6 +117,72 @@ class Akaze:
                                                     desc.ctypes.data, cap, n.ctypes.data))
         return [kp[b, :n[b]].copy() for b in range(B)], [desc[b, :n[b]].copy() for b in range(B)]
 
+    # -- the staged surface (akaze/src/lib.rs:341-345; include/cvb200_stages.h)
+    def create_scale_space(self, images):
+        """allocate_evolutions + create_nonlinear_scale_space + detector_response of [H, W] or [B, H, W] frames, resident on the
+        device: float32 as it is, uint8 / uint16 converted as `extract` converts them.  Returns a ScaleSpace, which any later call
+        that rewrites this context's AKAZE planes (an extract, another scale space) makes stale."""
+        images = np.asarray(images)
+        if images.dtype == np.uint8:
+            images = images.astype(np.float32) / np.float32(255)
+        elif images.dtype == np.uint16:
+            images = images.astype(np.float32) / np.float32(65535)
+        elif images.dtype != np.float32:
+            raise TypeError("images must be float32, uint8 or uint16")
+        if images.ndim == 2:
+            images = images[None]
+        if images.ndim != 3:
+            raise ValueError("images must be [H, W] or [B, H, W]")
+        images = np.ascontiguousarray(images)
+        B, H, W = images.shape
+        ctx = self._ctx()
+        L = load_stages_library()
+        ticket = C.c_uint64()
+        ctx.check(L.cvb_akaze_scale_space(ctx.handle, C.byref(self.config.to_c()), images.ctypes.data, B, W, H, C.byref(ticket)))
+        return ScaleSpace(ctx, ticket.value, B, W, H, self.config)
+
+    def find_image_keypoints(self, scale_space):
+        """Akaze::find_image_keypoints (lib.rs:268-276) on a ScaleSpace: per frame, the keypoints in the reference's order, neither
+        sorted nor truncated (maximum_features is ignored, as in the reference).  Detection runs with the config the scale space was
+        built with (its detector response already depends on it), so this Akaze's detector fields must equal that config's:
+        ValueError otherwise.  Only maximum_features and the descriptor fields may differ."""
+        mine, built = _detector_fields(self.config), _detector_fields(scale_space.config)
+        if mine != built:
+            raise ValueError(f"detector config {mine} differs from the scale space's {built}: build the scale space with this Akaze")
+        ctx, L = scale_space.ctx, load_stages_library()
+        cap = max(self.max_keypoints, 1)
+        while True:
+            kp = np.zeros((scale_space.batch, cap), dtype=KP_DTYPE)
+            n = np.zeros(scale_space.batch, dtype=np.uint32)
+            rc = L.cvb_akaze_find_image_keypoints(ctx.handle, scale_space.ticket, kp.ctypes.data, cap, n.ctypes.data)
+            if rc == CVB_ECAP and int(n.max()) > cap:
+                cap = int(n.max())
+                continue
+            ctx.check(rc)
+            return [kp[b, :n[b]].copy() for b in range(scale_space.batch)]
+
+    def extract_descriptors(self, scale_space, keypoints_per_frame):
+        """Akaze::extract_descriptors(&evolutions, &keypoints) (descriptors.rs:16-45) for one keypoint array per frame of the scale
+        space (a bare array when it has one frame).  Only descriptor_channels and descriptor_pattern_size of this Akaze are read.
+        Returns per-frame lists (keypoints kept, in input order; their [n, 64] uint8 descriptors)."""
+        if isinstance(keypoints_per_frame, np.ndarray) and keypoints_per_frame.dtype == KP_DTYPE:
+            keypoints_per_frame = [keypoints_per_frame]
+        frames = [np.ascontiguousarray(k, dtype=KP_DTYPE).reshape(-1) for k in keypoints_per_frame]
+        if len(frames) != scale_space.batch:
+            raise ValueError(f"expected {scale_space.batch} keypoint arrays, got {len(frames)}")
+        offsets = np.zeros(len(frames) + 1, np.uint32)
+        offsets[1:] = np.cumsum([len(k) for k in frames])
+        kp_in = np.concatenate(frames) if offsets[-1] else np.zeros(1, KP_DTYPE)
+        total = max(int(offsets[-1]), 1)
+        kp_out = np.zeros(total, KP_DTYPE)
+        desc = np.zeros((total, 64), np.uint8)
+        n = np.zeros(len(frames), np.uint32)
+        ctx, L = scale_space.ctx, load_stages_library()
+        ctx.check(L.cvb_akaze_extract_descriptors(ctx.handle, C.byref(self.config.to_c()), scale_space.ticket, kp_in.ctypes.data,
+                                                  offsets.ctypes.data, kp_out.ctypes.data, desc.ctypes.data, n.ctypes.data))
+        return ([kp_out[offsets[b]:offsets[b] + n[b]].copy() for b in range(len(frames))],
+                [desc[offsets[b]:offsets[b] + n[b]].copy() for b in range(len(frames))])
+
     # -- introspection used by the parity tests (no reference counterpart)
     def debug_evolutions(self):
         ctx = self._ctx()
@@ -151,4 +217,27 @@ class Akaze:
         return out[:n.value]
 
 
-__all__ = ["Akaze", "AkazeConfig", "CvbError", "Context"]
+def _detector_fields(config):
+    """the AkazeConfig fields find_image_keypoints depends on: all but maximum_features (ignored by find), the two descriptor
+    fields (read by describe only) and initial_contrast (never read, lib.rs:123,176)"""
+    skip = {"maximum_features", "descriptor_channels", "descriptor_pattern_size", "initial_contrast"}
+    return {f: v for f, v in asdict(config).items() if f not in skip}
+
+
+class ScaleSpace:
+    """A scale space resident in a context's AKAZE workspace (the device-side counterpart of akaze's Vec<EvolutionStep>):
+    `ticket` names it in include/cvb200_stages.h, `evolutions` is its EvolutionStep table (EVOLUTION_DTYPE), `config` the
+    AkazeConfig it was built with."""
+
+    def __init__(self, ctx, ticket, batch, width, height, config):
+        self.ctx, self.ticket, self.batch, self.width, self.height = ctx, ticket, batch, width, height
+        self.config = replace(config)
+        L = load_stages_library()
+        n = C.c_uint32()
+        ctx.check(L.cvb_akaze_evolutions(ctx.handle, ticket, None, 0, C.byref(n)))
+        self.evolutions = np.zeros(n.value, EVOLUTION_DTYPE)
+        if n.value:
+            ctx.check(L.cvb_akaze_evolutions(ctx.handle, ticket, self.evolutions.ctypes.data, n.value, C.byref(n)))
+
+
+__all__ = ["Akaze", "AkazeConfig", "CvbError", "Context", "ScaleSpace"]

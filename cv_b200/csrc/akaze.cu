@@ -8,7 +8,9 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <atomic>
 #include <vector>
+#include "../../include/cvb200_stages.h"
 #include "akaze_kernels.cuh"
 #include "common.cuh"
 
@@ -162,6 +164,17 @@ struct AkazeWorkspace {
     uint64_t launches_per_graph = 0;
     bool use_graph = true;       // CVB_NO_GRAPH=1 disables
     bool use_aux = true;         // CVB_NO_AUX_STREAM=1 disables
+    // staged calls (include/cvb200_stages.h): the ticket of the scale space the planes hold (0: none; an extract or a rebuild
+    // replaces the planes and so clears it) and its batch
+    uint64_t ticket = 0;
+    unsigned ss_batch = 0;
+    DescTables *dt_side = nullptr;   // descriptor tables of a describe config other than the workspace's own
+    int dt_side_pattern = 0, dt_side_nch = 0;
+    // grow-only buffers of the staged calls, sized by the call
+    cvb_keypoint *st_kp = nullptr, *st_kp_out = nullptr;
+    unsigned char *st_ok = nullptr, *st_desc = nullptr, *st_desc_out = nullptr;
+    unsigned *st_off = nullptr, *st_n = nullptr, *st_need = nullptr;
+    size_t st_kp_n = 0, st_kp_out_n = 0, st_ok_n = 0, st_desc_n = 0, st_desc_out_n = 0, st_off_n = 0, st_n_n = 0, st_need_n = 0;
 };
 
 void akaze_workspace_free(AkazeWorkspace *ws) {
@@ -171,6 +184,9 @@ void akaze_workspace_free(AkazeWorkspace *ws) {
     for (cudaEvent_t e : ws->ev_fork) if (e) cudaEventDestroy(e);
     if (ws->ev_join) cudaEventDestroy(ws->ev_join);
     for (void *p : ws->allocs) cudaFree(p);
+    for (void *p : {(void *)ws->st_kp, (void *)ws->st_kp_out, (void *)ws->st_ok, (void *)ws->st_desc, (void *)ws->st_desc_out,
+                    (void *)ws->st_off, (void *)ws->st_n, (void *)ws->st_need})
+        if (p) cudaFree(p);
     delete ws;
 }
 
@@ -287,6 +303,44 @@ int plan_evolutions(cvb_ctx *ctx, AkazeWorkspace *ws) {
     return 0;
 }
 
+// descriptor tables (descriptors.rs:64-96,117-124,188-201) of one (descriptor_pattern_size, descriptor_channels)
+int make_desc_tables(cvb_ctx *ctx, int pattern, int nch, DescTables *dt) {
+    memset(dt, 0, sizeof(*dt));
+    if (pattern < 1 || pattern > DESC_MAXLAT) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %d out of range", pattern);
+    const float size_mult[3] = {1.0f, 2.0f / 3.0f, 1.0f / 2.0f};
+    int base[3], ncell = 0;
+    for (int lvl = 0; lvl < 3; lvl++) {
+        int step = (int)ceilf((float)pattern * size_mult[lvl]);
+        base[lvl] = ncell;
+        int per_axis = 0;
+        for (int i = -pattern; i < pattern; i += step) per_axis++;
+        if (per_axis != lvl + 2) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %d: grid %d has %d cells per axis", pattern, lvl, per_axis);
+        for (int i = -pattern; i < pattern; i += step)
+            for (int j = -pattern; j < pattern; j += step) {
+                dt->ci[ncell] = (short)i; dt->cj[ncell] = (short)j; dt->cstep[ncell] = (short)step;
+                ncell++;
+            }
+    }
+    dt->ncells = ncell;
+    int kmax = -pattern;
+    for (int c = 0; c < ncell; c++) kmax = std::max(kmax, dt->ci[c] + dt->cstep[c] - 1);
+    dt->nlat = kmax + pattern + 1;
+    if (dt->nlat > DESC_MAXLAT) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %d needs a %d-point lattice (max %d)", pattern, dt->nlat, DESC_MAXLAT);
+    int bit = 0;
+    for (int lvl = 0; lvl < 3; lvl++) {
+        int count = (lvl + 2) * (lvl + 2);
+        for (int pos = 0; pos < nch; pos++)
+            for (int a = 0; a < count; a++)
+                for (int b2 = a + 1; b2 < count; b2++) {
+                    dt->ba[bit] = (unsigned char)(base[lvl] + a); dt->bb[bit] = (unsigned char)(base[lvl] + b2);
+                    dt->bch[bit] = (unsigned char)pos;
+                    bit++;
+                }
+    }
+    dt->nbits = bit;
+    return 0;
+}
+
 int build_tables(cvb_ctx *ctx, AkazeWorkspace *ws) {
     // orientation tables (scale_space_extrema.rs:233-287)
     OrientTables ot;
@@ -335,42 +389,9 @@ int build_tables(cvb_ctx *ctx, AkazeWorkspace *ws) {
         if (!ok) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "orientation window table is not ordered as expected");
     }
     CVB_CUDA(ctx, cudaMemcpyAsync(ws->ot, &ot, sizeof(ot), cudaMemcpyHostToDevice, ctx->stream));
-    // descriptor tables (descriptors.rs:64-96,117-124,188-201)
     DescTables dt;
-    memset(&dt, 0, sizeof(dt));
-    const int pattern = (int)ws->cfg.descriptor_pattern_size, nch = (int)ws->cfg.descriptor_channels;
-
-    const float size_mult[3] = {1.0f, 2.0f / 3.0f, 1.0f / 2.0f};
-    int base[3], ncell = 0;
-    for (int lvl = 0; lvl < 3; lvl++) {
-        int step = (int)ceilf((float)pattern * size_mult[lvl]);
-        base[lvl] = ncell;
-        int per_axis = 0;
-        for (int i = -pattern; i < pattern; i += step) per_axis++;
-        if (per_axis != lvl + 2) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %d: grid %d has %d cells per axis", pattern, lvl, per_axis);
-        for (int i = -pattern; i < pattern; i += step)
-            for (int j = -pattern; j < pattern; j += step) {
-                dt.ci[ncell] = (short)i; dt.cj[ncell] = (short)j; dt.cstep[ncell] = (short)step;
-                ncell++;
-            }
-    }
-    dt.ncells = ncell;
-    int kmax = -pattern;
-    for (int c = 0; c < ncell; c++) kmax = std::max(kmax, dt.ci[c] + dt.cstep[c] - 1);
-    dt.nlat = kmax + pattern + 1;
-    if (dt.nlat > DESC_MAXLAT) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %d needs a %d-point lattice (max %d)", pattern, dt.nlat, DESC_MAXLAT);
-    int bit = 0;
-    for (int lvl = 0; lvl < 3; lvl++) {
-        int count = (lvl + 2) * (lvl + 2);
-        for (int pos = 0; pos < nch; pos++)
-            for (int a = 0; a < count; a++)
-                for (int b2 = a + 1; b2 < count; b2++) {
-                    dt.ba[bit] = (unsigned char)(base[lvl] + a); dt.bb[bit] = (unsigned char)(base[lvl] + b2);
-                    dt.bch[bit] = (unsigned char)pos;
-                    bit++;
-                }
-    }
-    dt.nbits = bit;
+    int rc = make_desc_tables(ctx, (int)ws->cfg.descriptor_pattern_size, (int)ws->cfg.descriptor_channels, &dt);
+    if (rc) return rc;
     CVB_CUDA(ctx, cudaMemcpyAsync(ws->dt, &dt, sizeof(dt), cudaMemcpyHostToDevice, ctx->stream));
     std::vector<int> oct(MAX_EVO, 0);
     for (size_t i = 0; i < ws->evo.size(); i++) oct[i] = (int)ws->evo[i].octave;
@@ -452,7 +473,7 @@ int build_workspace(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, 
         cudaEventCreateWithFlags(&ws->ev_join, cudaEventDisableTiming);
         cudaFuncSetAttribute(k_suppress_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SUP_SMEM);
     }
-    DA(ot, 1); DA(dt, 1);
+    DA(ot, 1); DA(dt, 1); DA(dt_side, 1);
     DA(tmaps, 3 * MAX_EVO);
     DA(kp_out, B * (size_t)cap_out); DA(desc_out, B * (size_t)cap_out * 64); DA(n_out, B);
 #undef DA
@@ -567,19 +588,18 @@ int launch_deriv2(cvb_ctx *ctx, const EvoHost &e, const float *Lx, const float *
     return 0;
 }
 
-// The whole extractor for `B` frames already resident in `images` (device).  Asynchronous.
-int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoint *kp_out, unsigned char *desc_out,
-                      unsigned cap_out, unsigned *n_out) {
+// ---- the extractor in three stages (lib.rs:309-339), each asynchronous on the context's stream and for B >= 1 frames of a
+// workspace with at least one evolution.  run_extract_eager issues them in order; the staged calls of include/cvb200_stages.h
+// issue them one at a time.
+
+// create_nonlinear_scale_space + detector_response (lib.rs:193-258, detector_response.rs:8-85) for `B` frames already resident
+// in `images` (device): every plane, and the extrema mask and per-row counts of the fused detector response
+int stage_scale_space(cvb_ctx *ctx, const float *images, unsigned B) {
     AkazeWorkspace *ws = ctx->akaze;
     cudaStream_t st = ctx->stream;
     const size_t PF = ws->plane_floats, P0 = ws->p0;
     const int W = (int)ws->w, H = (int)ws->h;
     const int E = (int)ws->evo.size();
-    if (E == 0) {   // image too small for a single octave: the reference returns no keypoints
-        CVB_CUDA(ctx, cudaMemsetAsync(n_out, 0, sizeof(unsigned) * B, st));
-        ws->has_run = true;
-        return 0;
-    }
     const int nbins = (int)ws->cfg.contrast_factor_num_bins;
     int smax = 1;
     for (const EvoHost &e : ws->evo) smax = std::max(smax, (int)e.sigma);
@@ -727,7 +747,18 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
         CVB_CUDA(ctx, cudaEventRecord(ws->ev_join, ws->aux));
         CVB_CUDA(ctx, cudaStreamWaitEvent(st, ws->ev_join, 0));
     }
-    // ---- detect_keypoints (scale_space_extrema.rs)
+    return 0;
+}
+
+// detect_keypoints (scale_space_extrema.rs): find_scale_space_extrema + do_subpixel_refinement on the planes of
+// stage_scale_space; leaves ncache[b] keypoints per frame in `refined`, valid[] marking the kept ones (the reference's order)
+int stage_detect(cvb_ctx *ctx, unsigned B) {
+    AkazeWorkspace *ws = ctx->akaze;
+    cudaStream_t st = ctx->stream;
+    const size_t PF = ws->plane_floats;
+    const bool fused_det = ws->deriv_v3 && ws->fuse_det;   // the detector response wrote the extrema mask itself
+    const int R = ws->table.total_rows;
+    const float thr = (float)ws->cfg.detector_threshold;
     {
         if (!fused_det) { CVB_PROF(ctx, "k_extrema_mask", 4.0 * ws->plane_floats * B);
         k_extrema_mask<<<dim3((unsigned)ws->table.total_tiles, 1, B), NT, 0, st>>>(ws->Ldet, PF, ws->table, ws->tile_evo, ws->mask_layout, thr,
@@ -762,7 +793,16 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
     k_refine_orient<<<dim3(kp_blocks, B), NT, 0, st>>>(ws->cache, ws->ncache, ws->capk, ws->keep, ws->table, ws->Ldet, ws->Lx, ws->Ly, PF,
                                                        ws->ot, ws->refined, ws->valid);
     CVB_LAUNCH_CHECK(ctx); }
-    // ---- sort + truncate (lib.rs:326-327)
+    return 0;
+}
+
+// sort + truncate (lib.rs:326-327) and extract_descriptors (descriptors.rs:16-45) of stage_detect's keypoints, compacted into
+// the caller's B x cap_out outputs
+int stage_sort_describe(cvb_ctx *ctx, unsigned B, cvb_keypoint *kp_out, unsigned char *desc_out, unsigned cap_out, unsigned *n_out) {
+    AkazeWorkspace *ws = ctx->akaze;
+    cudaStream_t st = ctx->stream;
+    const size_t PF = ws->plane_floats;
+    const unsigned ichunks = std::min<unsigned>(cdiv(ws->capk, NT), 64u);
     CVB_CUDA(ctx, cudaMemsetAsync(ws->rank, 0, sizeof(unsigned) * (size_t)B * ws->capk, st));
     CVB_CUDA(ctx, cudaMemsetAsync(ws->nvalid, 0, sizeof(unsigned) * B, st));
     { CVB_PROF(ctx, "k_rank_sort", 0);
@@ -775,14 +815,30 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
     CVB_LAUNCH_CHECK(ctx); }
     // ---- extract_descriptors (descriptors.rs:16-45)
     { CVB_PROF(ctx, "k_descriptors", 0);
-    k_descriptors<<<dim3((unsigned)ctx->num_sms * 8, B), DESC_WARPS * 32, 0, st>>>(ws->sorted, ws->nsorted, ws->capk, ws->table, ws->Lt, ws->Lx,
-                                                     ws->Ly, PF, ws->dt, (int)ws->cfg.descriptor_channels,
-                                                     (int)ws->cfg.descriptor_pattern_size, ws->desc_tmp, ws->ok);
+    k_descriptors<<<dim3((unsigned)ctx->num_sms * 8, B), DESC_WARPS * 32, 0, st>>>(ws->sorted, ws->nsorted, nullptr, ws->capk, ws->table, ws->Lt,
+                                                     ws->Lx, ws->Ly, PF, ws->dt, (int)ws->cfg.descriptor_channels,
+                                                     (int)ws->cfg.descriptor_pattern_size, ws->desc_tmp, ws->ok, ws->overflow);
     CVB_LAUNCH_CHECK(ctx); }
     { CVB_PROF(ctx, "k_compact_final", 0);
     k_compact_final<<<B, 1024, 0, st>>>(ws->sorted, ws->desc_tmp, ws->ok, ws->nsorted, ws->capk, kp_out, desc_out, cap_out, n_out,
                                         ws->overflow);
     CVB_LAUNCH_CHECK(ctx); }
+    return 0;
+}
+
+// The whole extractor for `B` frames already resident in `images` (device).  Asynchronous.
+int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoint *kp_out, unsigned char *desc_out,
+                      unsigned cap_out, unsigned *n_out) {
+    AkazeWorkspace *ws = ctx->akaze;
+    if (ws->evo.empty()) {   // image too small for a single octave: the reference returns no keypoints
+        CVB_CUDA(ctx, cudaMemsetAsync(n_out, 0, sizeof(unsigned) * B, ctx->stream));
+        ws->has_run = true;
+        return 0;
+    }
+    int rc = stage_scale_space(ctx, images, B);
+    if (!rc) rc = stage_detect(ctx, B);
+    if (!rc) rc = stage_sort_describe(ctx, B, kp_out, desc_out, cap_out, n_out);
+    if (rc) return rc;
     ws->has_run = true;
     return 0;
 }
@@ -792,6 +848,7 @@ int run_extract_eager(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoin
 int run_extract(cvb_ctx *ctx, const float *images, unsigned B, cvb_keypoint *kp_out, unsigned char *desc_out,
                 unsigned cap_out, unsigned *n_out) {
     AkazeWorkspace *ws = ctx->akaze;
+    ws->ticket = 0;   // the planes no longer hold a staged scale space
     if (!ws->use_graph || ctx->prof || ws->evo.empty()) return run_extract_eager(ctx, images, B, kp_out, desc_out, cap_out, n_out);
     for (auto &g : ws->graphs)
         if (g.img == images && g.kp == kp_out && g.desc == desc_out && g.n == n_out && g.B == B && g.cap == cap_out) {
@@ -914,6 +971,211 @@ int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float
                                       cudaMemcpyDeviceToHost, st));
         CVB_CUDA(ctx, cudaMemcpyAsync(desc_out + (size_t)b * cap * 64, ws->desc_out + (size_t)b * cap_dev * 64, (size_t)n * 64,
                                       cudaMemcpyDeviceToHost, st));
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+// ---- staged calls: the bodies of include/cvb200_stages.h (exported by stages_abi.cu, libcvb200_stages.so) ---------------------
+
+namespace {
+
+std::atomic<uint64_t> g_scale_space_tickets{0};   // process-wide, so that a ticket of one context is unknown to every other
+
+int check_ticket(cvb_ctx *ctx, uint64_t ticket) {
+    if (!ctx) return CVB_EINVAL;
+    if (!ticket || !ctx->akaze || ctx->akaze->ticket != ticket)
+        return cvb_set_error(ctx, CVB_EINVAL, "scale space replaced: the ticket is stale or unknown to this context");
+    return 0;
+}
+
+// the descriptor tables of a describe config: the workspace's own when the config matches the scale space's, else side tables
+// built on demand (the scale space and its ticket stay as they are)
+int desc_tables_for(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, const DescTables **out) {
+    if (cfg->descriptor_channels < 1 || cfg->descriptor_channels > 3) return cvb_set_error(ctx, CVB_EINVAL, "descriptor_channels must be 1..3");
+    if (cfg->descriptor_pattern_size == ws->cfg.descriptor_pattern_size && cfg->descriptor_channels == ws->cfg.descriptor_channels) {
+        *out = ws->dt;
+        return 0;
+    }
+    if (cfg->descriptor_pattern_size > (uint64_t)DESC_MAXLAT)
+        return cvb_set_error(ctx, CVB_EUNSUPPORTED, "descriptor_pattern_size %llu out of range", (unsigned long long)cfg->descriptor_pattern_size);
+    const int pattern = (int)cfg->descriptor_pattern_size, nch = (int)cfg->descriptor_channels;
+    if (ws->dt_side_pattern != pattern || ws->dt_side_nch != nch) {
+        DescTables dt;
+        int rc = make_desc_tables(ctx, pattern, nch, &dt);
+        if (rc) return rc;
+        CVB_CUDA(ctx, cudaMemcpyAsync(ws->dt_side, &dt, sizeof(dt), cudaMemcpyHostToDevice, ctx->stream));
+        CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+        ws->dt_side_pattern = pattern; ws->dt_side_nch = nch;
+    }
+    *out = ws->dt_side;
+    return 0;
+}
+
+}  // namespace
+
+int stages_scale_space(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, bool on_device, uint32_t batch, uint32_t w,
+                       uint32_t h, uint64_t *ticket_out) {
+    int rc = check_args(ctx, cfg, images, batch, w, h);
+    if (rc) return rc;
+    if (!ticket_out) return cvb_set_error(ctx, CVB_EINVAL, "null output");
+    *ticket_out = 0;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    rc = ensure_workspace(ctx, cfg, batch, w, h, ctx->akaze ? ctx->akaze->cap_out : 1);
+    if (rc) return rc;
+    AkazeWorkspace *ws = ctx->akaze;
+    ws->ticket = 0;
+    if (!on_device) CVB_CUDA(ctx, cudaMemcpyAsync(ws->img, images, sizeof(float) * ws->p0 * batch, cudaMemcpyHostToDevice, ctx->stream));
+    if (!ws->evo.empty()) {
+        rc = stage_scale_space(ctx, on_device ? images : ws->img, batch);
+        if (rc) return rc;
+    }
+    if (!on_device) CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    ws->ss_batch = batch;
+    ws->ticket = ++g_scale_space_tickets;
+    *ticket_out = ws->ticket;
+    return 0;
+}
+
+int stages_evolutions(cvb_ctx *ctx, uint64_t ticket, cvb_akaze_evolution *out, uint32_t cap, uint32_t *n_out) {
+    int rc = check_ticket(ctx, ticket);
+    if (rc) return rc;
+    if (!n_out || (cap && !out)) return cvb_set_error(ctx, CVB_EINVAL, "null output");
+    const AkazeWorkspace *ws = ctx->akaze;
+    *n_out = (uint32_t)ws->evo.size();
+    for (size_t i = 0; i < ws->evo.size() && i < cap; i++) {
+        const EvoHost &e = ws->evo[i];
+        // sigma_size is EvolutionStep's `esigma.round() as u32` (evolution.rs:58; round() is half away from zero), not the
+        // derivative scale of the detector response (EvoHost::sigma, detector_response.rs:13)
+        out[i] = cvb_akaze_evolution{e.octave, e.sublevel, e.esigma, e.etime, (uint32_t)round(e.esigma), (uint32_t)e.w, (uint32_t)e.h,
+                                     (uint32_t)e.tau.size()};
+    }
+    return 0;
+}
+
+int stages_find(cvb_ctx *ctx, uint64_t ticket, cvb_keypoint *kp_out, uint32_t cap, uint32_t *n_out, bool on_device) {
+    int rc = check_ticket(ctx, ticket);
+    if (rc) return rc;
+    if (!n_out || (cap && !kp_out)) return cvb_set_error(ctx, CVB_EINVAL, "null output");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    AkazeWorkspace *ws = ctx->akaze;
+    cudaStream_t st = ctx->stream;
+    const unsigned B = ws->ss_batch;
+    if (ws->evo.empty()) {   // no octave: no keypoints (lib.rs:268-276 over an empty evolution table)
+        if (on_device) CVB_CUDA(ctx, cudaMemsetAsync(n_out, 0, sizeof(unsigned) * B, st));
+        else memset(n_out, 0, sizeof(unsigned) * B);
+        return 0;
+    }
+    // detection runs on every call, so that every find reports its own capacity overflows (flags 1 and 2).  It reads the planes
+    // and the per-row extrema counts of the scale space; the unfused extrema mask adds to those counts, so they restart from 0.
+    if (!(ws->deriv_v3 && ws->fuse_det))
+        CVB_CUDA(ctx, cudaMemsetAsync(ws->rowcount, 0, sizeof(unsigned) * (size_t)B * ws->table.total_rows, st));
+    if ((rc = stage_detect(ctx, B))) return rc;
+    CompactArgs A{};
+    A.kp_in = ws->refined; A.keep = ws->valid; A.counts = ws->ncache; A.in_stride = ws->capk; A.cap = cap;
+    A.overflow = ws->overflow;
+    if (on_device) {
+        A.kp_out = kp_out; A.n_out = n_out;
+    } else {
+        if ((rc = ws_grow(ctx, &ws->st_kp_out, &ws->st_kp_out_n, (size_t)B * cap))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_n, &ws->st_n_n, B))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_need, &ws->st_need_n, B))) return rc;
+        A.kp_out = ws->st_kp_out; A.n_out = ws->st_n; A.need = ws->st_need;
+    }
+    { CVB_PROF(ctx, "k_compact_stage", 0);
+    k_compact_stage<<<B, 1024, 0, st>>>(A);
+    CVB_LAUNCH_CHECK(ctx); }
+    if (on_device) return 0;
+    unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * (2 * (size_t)B + 1));
+    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->st_n, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs + B, ws->st_need, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs + 2 * B, ws->overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    const unsigned ovf = hs[2 * B];
+    std::vector<unsigned> got(hs, hs + B), need(hs + B, hs + 2 * B);
+    if (ovf) CVB_CUDA(ctx, cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st));
+    if (ovf == 1 || ovf == 2) return cvb_set_error(ctx, CVB_ECAP, "internal keypoint capacity exceeded (stage %u)", ovf);
+    for (unsigned b = 0; b < B; b++)
+        if (need[b] > cap) {
+            for (unsigned c = 0; c < B; c++) n_out[c] = need[c];
+            return cvb_set_error(ctx, CVB_ECAP, "output capacity %u too small: frame %u has %u keypoints", cap, b, need[b]);
+        }
+    for (unsigned b = 0; b < B; b++) {
+        n_out[b] = got[b];
+        if (got[b])
+            CVB_CUDA(ctx, cudaMemcpyAsync(kp_out + (size_t)b * cap, ws->st_kp_out + (size_t)b * cap, sizeof(cvb_keypoint) * got[b],
+                                          cudaMemcpyDeviceToHost, st));
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int stages_describe(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, uint64_t ticket, const cvb_keypoint *kp_in, const uint32_t *offsets,
+                    uint32_t total_max, cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t *n_out, bool on_device) {
+    int rc = check_ticket(ctx, ticket);
+    if (rc) return rc;
+    if (!cfg || !offsets || !n_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    AkazeWorkspace *ws = ctx->akaze;
+    cudaStream_t st = ctx->stream;
+    const unsigned B = ws->ss_batch;
+    const DescTables *dt = nullptr;
+    if ((rc = desc_tables_for(ctx, ws, cfg, &dt))) return rc;
+    size_t total = total_max;
+    if (!on_device) {   // the checks the _dev kernel makes per keypoint, with the first offender named
+        for (unsigned b = 0; b < B; b++)
+            if (offsets[b] > offsets[b + 1]) return cvb_set_error(ctx, CVB_EINVAL, "offsets[%u] > offsets[%u]", b, b + 1);
+        total = offsets[B];
+        if (total > offsets[0] && !kp_in) return cvb_set_error(ctx, CVB_EINVAL, "null keypoint buffer");
+        const uint32_t E = (uint32_t)ws->evo.size();
+        for (size_t i = offsets[0]; i < total; i++) {
+            if (kp_in[i].class_id >= E)
+                return cvb_set_error(ctx, CVB_EINVAL, "keypoint %zu: class_id %u, the scale space has %u evolutions", i, kp_in[i].class_id, E);
+            if (kp_in[i].octave >= 32) return cvb_set_error(ctx, CVB_EINVAL, "keypoint %zu: octave %u >= 32", i, kp_in[i].octave);
+        }
+    }
+    if (total && (!kp_in || !kp_out || !desc_out)) return cvb_set_error(ctx, CVB_EINVAL, "null keypoint or descriptor buffer");
+    if (total > 0xffffffffull) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "too many keypoints");
+    if ((rc = ws_grow(ctx, &ws->st_ok, &ws->st_ok_n, total))) return rc;
+    if ((rc = ws_grow(ctx, &ws->st_desc, &ws->st_desc_n, total * 64))) return rc;
+    CompactArgs A{};
+    A.desc_in = ws->st_desc; A.keep = ws->st_ok; A.in_stride = (unsigned)total; A.overflow = ws->overflow;
+    const cvb_keypoint *kin = kp_in;
+    if (on_device) {
+        A.offs = offsets; A.kp_out = kp_out; A.desc_out = desc_out; A.n_out = n_out;
+    } else {
+        if ((rc = ws_grow(ctx, &ws->st_kp, &ws->st_kp_n, total))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_kp_out, &ws->st_kp_out_n, total))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_desc_out, &ws->st_desc_out_n, total * 64))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_off, &ws->st_off_n, (size_t)B + 1))) return rc;
+        if ((rc = ws_grow(ctx, &ws->st_n, &ws->st_n_n, B))) return rc;
+        if (total) CVB_CUDA(ctx, cudaMemcpyAsync(ws->st_kp, kp_in, sizeof(cvb_keypoint) * total, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(ws->st_off, offsets, sizeof(unsigned) * ((size_t)B + 1), cudaMemcpyHostToDevice, st));
+        kin = ws->st_kp;
+        A.offs = ws->st_off; A.kp_out = ws->st_kp_out; A.desc_out = ws->st_desc_out; A.n_out = ws->st_n;
+    }
+    A.kp_in = kin;
+    { CVB_PROF(ctx, "k_descriptors", 0);
+    k_descriptors<<<dim3((unsigned)ctx->num_sms * 8, B), DESC_WARPS * 32, 0, st>>>(kin, nullptr, A.offs, (unsigned)total, ws->table, ws->Lt,
+                                                     ws->Lx, ws->Ly, ws->plane_floats, dt, (int)cfg->descriptor_channels,
+                                                     (int)cfg->descriptor_pattern_size, ws->st_desc, ws->st_ok, ws->overflow);
+    CVB_LAUNCH_CHECK(ctx); }
+    { CVB_PROF(ctx, "k_compact_stage", 0);
+    k_compact_stage<<<B, 1024, 0, st>>>(A);
+    CVB_LAUNCH_CHECK(ctx); }
+    if (on_device) return 0;
+    unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * B);
+    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->st_n, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    std::vector<unsigned> got(hs, hs + B);
+    for (unsigned b = 0; b < B; b++) {
+        n_out[b] = got[b];
+        if (!got[b]) continue;
+        const size_t o = offsets[b];
+        CVB_CUDA(ctx, cudaMemcpyAsync(kp_out + o, ws->st_kp_out + o, sizeof(cvb_keypoint) * got[b], cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(desc_out + o * 64, ws->st_desc_out + o * 64, (size_t)got[b] * 64, cudaMemcpyDeviceToHost, st));
     }
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;

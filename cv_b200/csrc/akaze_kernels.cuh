@@ -1813,22 +1813,38 @@ constexpr int DESC_MAXLAT = 21;    // lattice points per axis: k, l in [-pattern
 // position depends on k and l only), so each lattice point is gathered ONCE per keypoint by the whole
 // warp (Lt, Lx, Ly and the rotated derivatives), parked in shared memory, and the per-cell sums then
 // read it back in the reference's k-outer / l-inner order -- same values, same order, 2.8x fewer gathers.
-__global__ void __launch_bounds__(DESC_WARPS * 32) k_descriptors(const cvb_keypoint *__restrict__ sorted,
-                                                    const unsigned *__restrict__ nsorted, unsigned capk, EvoTable T,
+// Frame b's keypoints are kps[base, base + n): base = b * stride and n = counts[b] when offs is null (the extractor's
+// per-frame slots); otherwise base = offs[b] and n = offs[b + 1] - base, both clamped to `stride` entries (caller keypoints
+// in CSR layout).  A keypoint with class_id >= T.n or octave >= 32 (an out-of-bounds index or a shift overflow in the
+// reference) gets ok = 0 and sets *flag = 4.
+__global__ void __launch_bounds__(DESC_WARPS * 32) k_descriptors(const cvb_keypoint *__restrict__ kps,
+                                                    const unsigned *__restrict__ counts, const unsigned *__restrict__ offs,
+                                                    unsigned stride, EvoTable T,
                                                     const float *__restrict__ Lt, const float *__restrict__ Lx,
                                                     const float *__restrict__ Ly, size_t bstride,
                                                     const DescTables *__restrict__ DT, int nch, int pattern,
                                                     unsigned char *__restrict__ desc_tmp,
-                                                    unsigned char *__restrict__ ok) {
+                                                    unsigned char *__restrict__ ok, unsigned *flag) {
     __shared__ float s_val[DESC_WARPS][32][3];
     __shared__ float s_lat[DESC_WARPS][3][DESC_MAXLAT * DESC_MAXLAT];
     const int b = blockIdx.y;
-    const unsigned n = nsorted[b];
+    size_t base;
+    unsigned n;
+    if (offs) {
+        const unsigned lo = min(offs[b], stride), hi = min(max(offs[b + 1], lo), stride);
+        base = lo; n = hi - lo;
+    } else {
+        base = (size_t)b * stride; n = counts[b];
+    }
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int nl = DT->nlat;                   // lattice size per axis (<= DESC_MAXLAT)
     for (unsigned q = blockIdx.x * DESC_WARPS + wid; q < n; q += gridDim.x * DESC_WARPS) {
-        const size_t gi = (size_t)b * capk + q;
-        const cvb_keypoint kp = sorted[gi];
+        const size_t gi = base + q;
+        const cvb_keypoint kp = kps[gi];
+        if (kp.class_id >= (unsigned)T.n || kp.octave >= 32u) {
+            if (lane == 0) { ok[gi] = 0; *flag = 4u; }
+            continue;
+        }
         const EvoDev ev = T.e[kp.class_id];
         const size_t poff = (size_t)b * bstride + ev.off;
         const float *PT = Lt + poff, *PX = Lx + poff, *PY = Ly + poff;
@@ -1859,7 +1875,10 @@ __global__ void __launch_bounds__(DESC_WARPS * 32) k_descriptors(const cvb_keypo
                     const float kf = (float)(ki - pattern), lf = (float)(lj - pattern);
                     const float sample_y = yf + (lf * co * scale + kf * si * scale);
                     const float sample_x = xf + (-lf * si * scale + kf * co * scale);
-                    const float ry_ = roundf(sample_y), rx_ = roundf(sample_x);
+                    // `f32::round(v) as isize` (descriptors.rs:129-130) saturates, and maps NaN to 0
+                    float ry_ = roundf(sample_y), rx_ = roundf(sample_x);
+                    if (ry_ != ry_) ry_ = 0.f;
+                    if (rx_ != rx_) rx_ = 0.f;
                     if (!(rx_ >= 0.f && rx_ < (float)W) || !(ry_ >= 0.f && ry_ < (float)H)) oob = true;
                     else g[u] = (size_t)(int)ry_ * W + (int)rx_;
                     slot[u] = ki * nl + lj;
@@ -1970,6 +1989,69 @@ __global__ void __launch_bounds__(1024) k_compact_final(const cvb_keypoint *__re
     }
     // the count never exceeds the capacity (the overflow flag reports the truncation): downstream kernels index by it
     if (threadIdx.x == 0) n_out[b] = min(s_carry, cap_out);
+}
+
+// Ordered compaction of caller-visible stage results, one block per frame.  Input entries in_base(b) + i for i < n(b) with
+// keep[...] set go, in input order, to out[out_base(b) + pos] (with their 64-byte descriptors when desc_in is non-null).
+//   find:     in_base = b * in_stride, n = counts[b]; out_base = b * cap; entries past cap are dropped and set *overflow = 3
+//   describe: in_base = out_base = offs[b] and n = offs[b + 1] - offs[b], clamped to in_stride entries (never past the input)
+// n_out[b] = the number kept (at most cap); need (optional) = the number that passed, capacity aside.
+struct CompactArgs {
+    const cvb_keypoint *kp_in;
+    const unsigned char *desc_in, *keep;
+    const unsigned *counts, *offs;
+    unsigned in_stride, cap;
+    cvb_keypoint *kp_out;
+    unsigned char *desc_out;
+    unsigned *n_out, *need, *overflow;
+};
+__global__ void __launch_bounds__(1024) k_compact_stage(CompactArgs A) {
+    __shared__ unsigned s_warp[32];
+    __shared__ unsigned s_carry;
+    const int b = blockIdx.x;
+    size_t in_base, out_base;
+    unsigned n, cap;
+    if (A.offs) {
+        const unsigned lo = min(A.offs[b], A.in_stride), hi = min(max(A.offs[b + 1], lo), A.in_stride);
+        in_base = out_base = lo; n = cap = hi - lo;
+    } else {
+        in_base = (size_t)b * A.in_stride; n = A.counts[b]; out_base = (size_t)b * A.cap; cap = A.cap;
+    }
+    if (threadIdx.x == 0) s_carry = 0;
+    __syncthreads();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    for (unsigned base = 0; base < n; base += 1024) {
+        const unsigned i = base + threadIdx.x;
+        const unsigned v = (i < n && A.keep[in_base + i]) ? 1u : 0u;
+        unsigned x = v;
+        for (int o = 1; o < 32; o <<= 1) { unsigned t = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += t; }
+        if (lane == 31) s_warp[wid] = x;
+        __syncthreads();
+        if (wid == 0) {
+            unsigned y = s_warp[lane], z = y;
+            for (int o = 1; o < 32; o <<= 1) { unsigned t = __shfl_up_sync(0xffffffffu, z, o); if (lane >= o) z += t; }
+            s_warp[lane] = z - y;
+        }
+        __syncthreads();
+        const unsigned pos = s_carry + s_warp[wid] + x - v;
+        if (v) {
+            if (pos < cap) {
+                A.kp_out[out_base + pos] = A.kp_in[in_base + i];
+                if (A.desc_in) {
+                    const uint4 *s = (const uint4 *)(A.desc_in + (in_base + i) * 64);
+                    uint4 *d = (uint4 *)(A.desc_out + (out_base + pos) * 64);
+                    d[0] = s[0]; d[1] = s[1]; d[2] = s[2]; d[3] = s[3];
+                }
+            } else *A.overflow = 3u;
+        }
+        __syncthreads();
+        if (threadIdx.x == 1023) s_carry = pos + v;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        A.n_out[b] = min(s_carry, cap);
+        if (A.need) A.need[b] = s_carry;
+    }
 }
 
 }  // namespace akz

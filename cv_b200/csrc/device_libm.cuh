@@ -8,12 +8,25 @@
 //                   of glibc's -mfma ifunc variant (explicit fma()).
 //   atanf/atan2f  : fdlibm single-precision code, no contraction.
 // This translation unit MUST be compiled with -fmad=false so that no other multiply-add is fused.
+// sinf_glibc / cosf_glibc are __host__ __device__ so that the same source can be checked against the host libm on a CPU
+// (host code must then be compiled with -ffp-contract=off).
 #pragma once
 #include <stdint.h>
+#include <string.h>
 
 namespace dlm {
 
-__device__ __forceinline__ float poly_sincos(double x, double x2, bool neg_cos, int n) {
+__host__ __device__ __forceinline__ uint32_t f32_bits(float x) {
+#ifdef __CUDA_ARCH__
+    return __float_as_uint(x);
+#else
+    uint32_t u;
+    memcpy(&u, &x, 4);
+    return u;
+#endif
+}
+
+__host__ __device__ __forceinline__ float poly_sincos(double x, double x2, bool neg_cos, int n) {
     const double C0 = 0x1p0, C1 = -0x1.ffffffd0c621cp-2, C2 = 0x1.55553e1068f19p-5, C3 = -0x1.6c087e89a359dp-10,
                  C4 = 0x1.99343027bf8c3p-16;
     const double S1 = -0x1.555545995a603p-3, S2 = 0x1.1107605230bc4p-7, S3 = -0x1.994eb3774cf24p-13;
@@ -34,9 +47,9 @@ __device__ __forceinline__ float poly_sincos(double x, double x2, bool neg_cos, 
     }
 }
 
-__device__ __forceinline__ uint32_t abstop12(float x) { return (__float_as_uint(x) >> 20) & 0x7ff; }
+__host__ __device__ __forceinline__ uint32_t abstop12(float x) { return (f32_bits(x) >> 20) & 0x7ff; }
 
-__device__ __forceinline__ double reduce_fast(double x, int *np) {
+__host__ __device__ __forceinline__ double reduce_fast(double x, int *np) {
     const double HPI_INV = 0x1.45F306DC9C883p+23, HPI = 0x1.921FB54442D18p0;
     double r = x * HPI_INV;
     int n = ((int32_t)r + 0x800000) >> 24;
@@ -44,29 +57,83 @@ __device__ __forceinline__ double reduce_fast(double x, int *np) {
     return fma(-(double)n, HPI, x);
 }
 
-// valid for |y| < 120 (callers pass angles in [0, 2pi))
-__device__ __forceinline__ float sinf_glibc(float y) {
+// 4/pi in 8-bit steps: entry i holds bits 8i .. 8i + 31 of the fraction, so every exponent has an aligned word.  Constant memory
+// on the device (a local array would be indexed from the stack), a plain table on the host.
+#define DLM_INV_PIO4 {0xa2,       0xa2f9,     0xa2f983,   0xa2f9836e, 0xf9836e4e, 0x836e4e44, 0x6e4e4415, 0x4e441529, \
+                      0x441529fc, 0x1529fc27, 0x29fc2757, 0xfc2757d1, 0x2757d1f5, 0x57d1f534, 0xd1f534dd, 0xf534ddc0, \
+                      0x34ddc0db, 0xddc0db62, 0xc0db6295, 0xdb629599, 0x6295993c, 0x95993c43, 0x993c4390, 0x3c439041}
+static __constant__ uint32_t inv_pio4_dev[24] = DLM_INV_PIO4;
+static const uint32_t inv_pio4_host[24] = DLM_INV_PIO4;
+#undef DLM_INV_PIO4
+
+// glibc's reduce_large (sysdeps/ieee754/flt-32/s_sincosf.h) for 120 <= |y| < inf: x * 4/pi in 62-bit fixed point from the 24-bit
+// mantissa times 96 bits of 4/pi chosen by the exponent; returns the remainder in [-pi/4, pi/4] and the quadrant in *np.
+__host__ __device__ __forceinline__ double reduce_large(uint32_t xi, int *np) {
+#ifdef __CUDA_ARCH__
+    const uint32_t *arr = &inv_pio4_dev[(xi >> 26) & 15];
+#else
+    const uint32_t *arr = &inv_pio4_host[(xi >> 26) & 15];
+#endif
+    const double PI63 = 0x1.921FB54442D18p-62;   // pi * 2^-64
+    const int shift = (xi >> 23) & 7;
+    xi = (xi & 0xffffff) | 0x800000;
+    xi <<= shift;
+    uint64_t res0 = (uint32_t)(xi * arr[0]);
+    const uint64_t res1 = (uint64_t)xi * arr[4];
+    const uint64_t res2 = (uint64_t)xi * arr[8];
+    res0 = (res2 >> 32) | (res0 << 32);
+    res0 += res1;
+    const uint64_t n = (res0 + (1ULL << 61)) >> 62;
+    res0 -= n << 62;
+    const double x = (double)(int64_t)res0;
+    *np = (int)n;
+    return x * PI63;
+}
+
+// glibc 2.39 sinf (s_sinf.c) over the whole float range: |y| < 120 reduces with reduce_fast, finite |y| >= 120 with reduce_large
+// (the input's sign folded into the quadrant), and +-inf / NaN give NaN
+__host__ __device__ __forceinline__ float sinf_glibc(float y) {
     double x = (double)y;
     if (abstop12(y) < abstop12(0x1.921FB6p-1f)) {
         if (abstop12(y) < abstop12(0x1p-12f)) return y;
         return poly_sincos(x, x * x, false, 0);
     }
     int n;
-    x = reduce_fast(x, &n);
-    double s = ((n & 3) == 1 || (n & 3) == 2) ? -1.0 : 1.0;
-    return poly_sincos(x * s, x * x, (n & 2) != 0, n);
+    if (abstop12(y) < abstop12(120.0f)) {
+        x = reduce_fast(x, &n);
+        double s = ((n & 3) == 1 || (n & 3) == 2) ? -1.0 : 1.0;
+        return poly_sincos(x * s, x * x, (n & 2) != 0, n);
+    }
+    if (abstop12(y) < abstop12(__builtin_huge_valf())) {
+        const uint32_t xi = f32_bits(y);
+        x = reduce_large(xi, &n);
+        const int q = n + (int)(xi >> 31);
+        double s = ((q & 3) == 1 || (q & 3) == 2) ? -1.0 : 1.0;
+        return poly_sincos(x * s, x * x, (q & 2) != 0, n);
+    }
+    return (y - y) / (y - y);
 }
 
-__device__ __forceinline__ float cosf_glibc(float y) {
+__host__ __device__ __forceinline__ float cosf_glibc(float y) {
     double x = (double)y;
     if (abstop12(y) < abstop12(0x1.921FB6p-1f)) {
         if (abstop12(y) < abstop12(0x1p-12f)) return 1.0f;
         return poly_sincos(x, x * x, false, 1);
     }
     int n;
-    x = reduce_fast(x, &n);
-    double s = ((n & 3) == 1 || (n & 3) == 2) ? -1.0 : 1.0;
-    return poly_sincos(x * s, x * x, (n & 2) != 0, n ^ 1);
+    if (abstop12(y) < abstop12(120.0f)) {
+        x = reduce_fast(x, &n);
+        double s = ((n & 3) == 1 || (n & 3) == 2) ? -1.0 : 1.0;
+        return poly_sincos(x * s, x * x, (n & 2) != 0, n ^ 1);
+    }
+    if (abstop12(y) < abstop12(__builtin_huge_valf())) {
+        const uint32_t xi = f32_bits(y);
+        x = reduce_large(xi, &n);
+        const int q = n + (int)(xi >> 31);
+        double s = ((q & 3) == 1 || (q & 3) == 2) ? -1.0 : 1.0;
+        return poly_sincos(x * s, x * x, (q & 2) != 0, n ^ 1);
+    }
+    return (y - y) / (y - y);
 }
 
 __device__ __forceinline__ float atanf_glibc(float x) {
