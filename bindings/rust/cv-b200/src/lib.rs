@@ -201,3 +201,6 @@ pub mod lsh;
 
 // ---- INTEGRATION.md section 2j (include/cvb200_stages.h) ----
 pub mod stages;
+
+// ---- INTEGRATION.md section 2k (include/cvb200_batch.h) ----
+pub mod batch;

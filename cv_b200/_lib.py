@@ -1,7 +1,7 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
-(include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h) and
-cv_b200/libcvb200_stages.so (include/cvb200_stages.h)."""
+(include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
+cv_b200/libcvb200_stages.so (include/cvb200_stages.h) and cv_b200/libcvb200_batch.so (include/cvb200_batch.h)."""
 import ctypes as C
 import os
 
@@ -106,6 +106,14 @@ STAGES_ABI_SYMBOLS = [
     "cvb_akaze_scale_space", "cvb_akaze_scale_space_dev", "cvb_akaze_evolutions", "cvb_akaze_find_image_keypoints",
     "cvb_akaze_find_image_keypoints_dev", "cvb_akaze_extract_descriptors", "cvb_akaze_extract_descriptors_dev",
 ]
+
+# every symbol include/cvb200_batch.h declares (B independent ARRSAC problems per launch), exported by libcvb200_batch.so; checked by
+# tests/test_abi_batch.py
+BATCH_ABI_SYMBOLS = [
+    "cvb_arrsac_batch_dev", "cvb_arrsac_batch", "cvb_arrsac_commit_rng_batch", "cvb_two_view_options_dev",
+]
+# CVB_ARRSAC_BATCH_MAX of include/cvb200_batch.h
+ARRSAC_BATCH_MAX = 64
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -286,6 +294,31 @@ def load_stages_library():
         L.cvb_akaze_extract_descriptors_dev.argtypes = [vp, C.POINTER(AkazeCfg), u64, vp, vp, u32, vp, vp, vp]
         _STAGES_LIB = L
     return _STAGES_LIB
+
+
+_BATCH_LIB = None
+
+
+def batch_lib_path():
+    return os.path.join(_HERE, "libcvb200_batch.so")
+
+
+def load_batch_library():
+    """Loads libcvb200_batch.so, the module of include/cvb200_batch.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _BATCH_LIB
+    if _BATCH_LIB is None:
+        load_library()
+        p = batch_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32, i32 = C.c_void_p, C.c_uint32, C.c_int32
+        L.cvb_arrsac_batch_dev.argtypes = [vp, vp, i32, i32, vp, vp, vp, u32, u32, vp, vp, vp, u32, vp, vp]
+        L.cvb_arrsac_batch.argtypes = [vp, vp, i32, i32, vp, vp, vp, u32, vp, vp, vp, vp, vp]
+        L.cvb_arrsac_commit_rng_batch.argtypes = [vp, vp, u32, vp]
+        L.cvb_two_view_options_dev.argtypes = [vp, vp, vp, vp, u32, u32, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp]
+        _BATCH_LIB = L
+    return _BATCH_LIB
 
 
 class Context:

@@ -26,12 +26,19 @@
 //   k_ars_final     inlier list of the winner.
 // The candidate table is double buffered (rows = pose + inlier count + inlier bit mask); every k_ars_book writes the
 // surviving rows in sorted order into the other buffer, so there is no free list and no indirection.
+//
+// Batches: one launch per stage serves B independent problems.  The one-CTA kernels (begin, sprt, book, final) run B CTAs and take
+// the problem from blockIdx.x; the estimate, score and resolve grids take it from blockIdx.y.  Problem pb owns ctl[pb] and the pb-th
+// slice of every workspace buffer (ars_ws: strides from the launch parameters), its own staged raw-draw stream, data rows
+// [pb * sdata, pb * sdata + n) and the pb-th share of the undecided-predicate queue.  A single problem is the batch of one: pb = 0
+// everywhere, so its addresses, launches and results are those of the unbatched driver.
 #pragma once
 
 #define ARS_SORT_CAP 4096u     // max_candidate_hypotheses + estimations_per_block * models_per_sample must fit
 #define ARS_BOOK_NT 1024
 #define ARS_BOOK_SMEM (14u * ARS_SORT_CAP)
-#define ARS_QCAP (1u << 20)    // queue of undecided predicates of a scoring stage (entries beyond it are evaluated in place)
+#define ARS_QCAP (1u << 20)    // queue of undecided predicates of a scoring stage (entries beyond it are evaluated in place); a batch of B
+                               // problems splits it, ARS_QCAP / B entries per problem and stage
 
 struct ArrsacCtl {
     uint32_t n, init_n, Mv, npass;
@@ -53,6 +60,7 @@ struct ArrsacCtl {
     uint32_t stat_skip;                      // new-model units written 0 by early rejection instead of scored
     uint32_t stat_blk_w0, stat_blk_lt32;     // blocks with new models scored under worst == 0 / under acc_hi - worst < 32
     uint32_t stat_blk_bar0;                  // blocks whose new samples were drawn but not estimated (worst >= acc_hi)
+    uint32_t retired;                        // k_ars_book has taken this problem off the batch's live count
 };
 
 struct ArrsacParams {            // launch-constant configuration (by value)
@@ -65,10 +73,29 @@ struct ArrsacParams {            // launch-constant configuration (by value)
     uint32_t prefix, cmin;       // initial scoring in two stages: all words for the first `prefix` samples; for the rest, words >= 1 only
                                  // when the first 32 data hold >= cmin inliers (the SPRT computes a missing word itself if it ever needs one)
     uint32_t early;              // block scoring stops scoring new models that can no longer beat the bar (k_ars_score phase 1)
+    uint32_t nraw;               // staged raw draws per problem
+    uint32_t qcap;               // queue entries per problem and scoring stage (ARS_QCAP / B)
+    uint32_t sdata;              // data rows per problem (problem pb's rows start at pb * sdata)
     float lr_thr, eps0, delta0;
     double thr;
     int row0;
 };
+
+// per-problem slice sizes of the workspace buffers, in elements (the host allocates B of each, the kernels offset by pb)
+struct ArsStrides {
+    size_t samples0, models0, nposes0, vm, rows2, tmasks, nnew, nposes_new, newmask, samples_new, queue, a, b;
+};
+__host__ __device__ __forceinline__ ArsStrides ars_strides(const ArrsacParams &P) {
+    ArsStrides s;
+    const size_t h0 = P.H0 ? P.H0 : 1, g = P.G ? P.G : 1, m0 = P.H0 ? (size_t)P.H0 * P.MM : 1;
+    s.samples0 = h0 * P.K; s.models0 = m0; s.nposes0 = h0; s.vm = m0 > ARS_SORT_CAP ? m0 : ARS_SORT_CAP;
+    s.rows2 = 2 * (size_t)P.rows; s.tmasks = s.rows2 * P.NW;
+    s.nnew = g * P.MM; s.nposes_new = g; s.newmask = s.nnew * P.NW; s.samples_new = g * P.K;
+    s.queue = 2 * (size_t)P.qcap;
+    s.a = 3 * (size_t)P.sdata; s.b = (P.kind == 1 ? 4 : 3) * (size_t)P.sdata;
+    return s;
+}
+
 
 __device__ __forceinline__ unsigned long long ars_globaltimer() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 __device__ __forceinline__ uint64_t ars_rotl64(uint64_t x, int k) { return (x << k) | (x >> (64 - k)); }
@@ -231,7 +258,9 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_begin(ArrsacCtl *ctl, Arrsa
                                                             const uint32_t *raw, uint32_t *samples0) {
     __shared__ uint32_t win[ARS_WIN];
     __shared__ __align__(8) uint32_t sh[4];
-    const uint32_t n = min(n_dev ? *n_dev : n_host, P.NMAX);
+    const uint32_t pb = blockIdx.x;
+    ctl += pb; raw += (size_t)pb * P.nraw; samples0 += pb * ars_strides(P).samples0;
+    const uint32_t n = min(n_dev ? n_dev[pb] : n_host, P.NMAX);
     if (threadIdx.x == 0) {
         ctl->n = n;
         ctl->init_n = min(P.bs * P.ib, n);
@@ -250,8 +279,16 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_begin(ArrsacCtl *ctl, Arrsa
 template <int KIND>
 __global__ void __launch_bounds__(128) k_ars_estimate(const ArrsacCtl *ctl, int phase, uint32_t H_init, const double *__restrict__ a,
                                                       const double *__restrict__ b, const uint32_t *__restrict__ samples,
-                                                      cvb_pose *poses, uint8_t *nposes, int row0) {
+                                                      cvb_pose *poses, uint8_t *nposes, int row0, ArrsacParams P) {
+    const uint32_t pb = blockIdx.y;
+    ctl += pb;
     if (ctl->done) return;
+    {
+        const ArsStrides S = ars_strides(P);
+        a += pb * S.a; b += pb * S.b;
+        samples += pb * (phase == 0 ? S.samples0 : S.samples_new); poses += pb * (phase == 0 ? S.models0 : S.nnew);
+        nposes += pb * (phase == 0 ? S.nposes0 : S.nposes_new);
+    }
     const uint32_t H = phase == 0 ? H_init : ctl->n_new;
     const uint32_t h = blockIdx.x * blockDim.x + threadIdx.x;
     if (h >= H) return;
@@ -269,8 +306,16 @@ __global__ void __launch_bounds__(128) k_ars_estimate(const ArrsacCtl *ctl, int 
 template <int EIGHT_LANES, int MINB>
 __global__ void __launch_bounds__(128, MINB) k_ars_estimate8(const ArrsacCtl *ctl, int phase, uint32_t H_init, const double *__restrict__ a,
                                                        const double *__restrict__ b, const uint32_t *__restrict__ samples,
-                                                       cvb_pose *poses, uint8_t *nposes) {
+                                                       cvb_pose *poses, uint8_t *nposes, ArrsacParams P) {
+    const uint32_t pb = blockIdx.y;
+    ctl += pb;
     if (ctl->done) return;
+    {
+        const ArsStrides S = ars_strides(P);
+        a += pb * S.a; b += pb * S.b;
+        samples += pb * (phase == 0 ? S.samples0 : S.samples_new); poses += pb * (phase == 0 ? S.models0 : S.nnew);
+        nposes += pb * (phase == 0 ? S.nposes0 : S.nposes_new);
+    }
     __shared__ double sh[(128 / EIGHT_LANES) * EIGHT_SH];
     const uint32_t H = phase == 0 ? H_init : ctl->n_new;
     const uint32_t g = threadIdx.x / EIGHT_LANES, lane = threadIdx.x % EIGHT_LANES;
@@ -308,13 +353,13 @@ __device__ __forceinline__ bool ars_inlier(const cvb_pose &Pz, const double *__r
 // Returns 1 (inlier), 0 (certain outlier) or -1 (queued: its mask bit is 0 until k_ars_resolve* decides it).
 template <int RES>
 __device__ __forceinline__ int ars_inlier_queued(const cvb_pose &Pz, const double *__restrict__ a, const double *__restrict__ b, uint32_t i,
-                                                 double thr, uint32_t *qc, uint2 *q, uint32_t src) {
+                                                 double thr, uint32_t *qc, uint2 *q, uint32_t qcap, uint32_t src) {
     if (RES == 1) return ars_inlier<RES>(Pz, a, b, i, thr) ? 1 : 0;
     const double *pa = a + 3 * (size_t)i, *pb = b + 3 * (size_t)i;
     const int f = c2c_inlier_filter(Pz.r, Pz.t, pa, pb, thr);
     if (f >= 0) return f != 0 ? 1 : 0;
     const uint32_t slot = atomicAdd(qc, 1u);
-    if (slot < ARS_QCAP) { q[slot] = make_uint2(src, i); return -1; }
+    if (slot < qcap) { q[slot] = make_uint2(src, i); return -1; }
     return ars_exact_c2c(&Pz, pa, pb, thr) ? 1 : 0;
 }
 
@@ -335,7 +380,15 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
                                                    const cvb_pose *__restrict__ tposes, uint32_t *__restrict__ tmasks,
                                                    const cvb_pose *__restrict__ newposes, const uint8_t *__restrict__ nposes_new,
                                                    uint32_t *__restrict__ newmask, uint32_t *nout) {
+    const uint32_t pb = blockIdx.y;
+    ctl += pb;
     if (ctl->done) return;
+    {
+        const ArsStrides S = ars_strides(P);
+        queue += pb * S.queue; a += pb * S.a; b += pb * S.b; poses0 += pb * S.models0; nposes0 += pb * S.nposes0;
+        masks0 += pb * S.models0 * P.W0; tposes += pb * S.rows2; tmasks += pb * S.tmasks; newposes += pb * S.nnew;
+        nposes_new += pb * S.nposes_new; newmask += pb * S.newmask; nout += pb * S.nnew;
+    }
     const unsigned full = 0xffffffffu;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -348,7 +401,7 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
         const uint32_t nmod = P.H0 * P.MM, npre = min(P.prefix, P.H0) * P.MM, W1 = W > 0 ? W - 1 : 0;
         const uint32_t units = phase == 0 ? nmod + npre * W1 : (nmod - npre) * W1;
         uint32_t *qc = phase == 0 ? &ctl->q_count : &ctl->q_count2;
-        uint2 *q = phase == 0 ? queue : queue + ARS_QCAP;
+        uint2 *q = phase == 0 ? queue : queue + P.qcap;
         for (uint32_t u = warp; u < units; u += nwarps) {
             uint32_t m, w;
             if (phase == 0) { if (u < nmod) { m = u; w = 0; } else { m = (u - nmod) / W1; w = 1 + (u - nmod) % W1; } }
@@ -357,7 +410,7 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
             if (phase == 2 && !ars_ready(masks0[(size_t)m * P.W0], init_n, m / P.MM, P)) continue;
             const uint32_t i = w * 32 + lane;
             bool bit = false;
-            if (i < init_n) bit = ars_inlier_queued<RES>(poses0[m], a, b, i, P.thr, qc, q, m) > 0;      // queue: k_ars_resolve
+            if (i < init_n) bit = ars_inlier_queued<RES>(poses0[m], a, b, i, P.thr, qc, q, P.qcap, m) > 0;      // queue: k_ars_resolve
             const unsigned bits = __ballot_sync(full, bit);
             if (lane == 0) { masks0[(size_t)m * P.W0 + w] = bits; atomicAdd(phase == 0 ? &ctl->stat_units0 : &ctl->stat_units2, 1u); }
         }
@@ -408,7 +461,7 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
         const uint32_t i = w * 32 + lane;
         const bool act = i < hi && (!kept || i >= lo);
         int f = -1;
-        if (act) f = ars_inlier_queued<RES>(kept ? tp[src] : newposes[src - P.rows], a, b, i, P.thr, &ctl->q_blk, queue, src);
+        if (act) f = ars_inlier_queued<RES>(kept ? tp[src] : newposes[src - P.rows], a, b, i, P.thr, &ctl->q_blk, queue, P.qcap, src);
         const unsigned bits = __ballot_sync(full, f > 0);
         if (kept) {
             const unsigned range = __ballot_sync(full, act);
@@ -429,9 +482,15 @@ __global__ void __launch_bounds__(256, 2) k_ars_score(ArrsacCtl *ctl, uint2 *__r
 __global__ void __launch_bounds__(256) k_ars_resolve(const ArrsacCtl *ctl, const uint2 *__restrict__ queue, int stage, ArrsacParams P,
                                                      const double *__restrict__ a, const double *__restrict__ b,
                                                      const cvb_pose *__restrict__ poses0, uint32_t *__restrict__ masks0) {
+    const uint32_t pb = blockIdx.y;
+    ctl += pb;
     if (ctl->done) return;
-    const uint32_t cnt = min(stage == 0 ? ctl->q_count : ctl->q_count2, ARS_QCAP);
-    queue += stage == 0 ? 0 : ARS_QCAP;
+    {
+        const ArsStrides S = ars_strides(P);
+        queue += pb * S.queue; a += pb * S.a; b += pb * S.b; poses0 += pb * S.models0; masks0 += pb * S.models0 * P.W0;
+    }
+    const uint32_t cnt = min(stage == 0 ? ctl->q_count : ctl->q_count2, P.qcap);
+    queue += stage == 0 ? 0 : P.qcap;
     for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < cnt; e += gridDim.x * blockDim.x) {
         const uint2 q = queue[e];
         if (residual_c2c(poses0[q.x], a + 3 * (size_t)q.y, b + 3 * (size_t)q.y) < P.thr)
@@ -445,8 +504,15 @@ __global__ void __launch_bounds__(64) k_ars_resolve_block(const ArrsacCtl *ctl, 
                                                           const double *__restrict__ a, const double *__restrict__ b,
                                                           const cvb_pose *__restrict__ tposes, uint32_t *__restrict__ tmasks,
                                                           const cvb_pose *__restrict__ newposes, uint32_t *__restrict__ newmask) {
+    const uint32_t pb = blockIdx.y;
+    ctl += pb;
     if (ctl->done) return;
-    const uint32_t cnt = min(ctl->q_blk, ARS_QCAP), cur = ctl->cur;
+    {
+        const ArsStrides S = ars_strides(P);
+        queue += pb * S.queue; a += pb * S.a; b += pb * S.b; tposes += pb * S.rows2; tmasks += pb * S.tmasks;
+        newposes += pb * S.nnew; newmask += pb * S.newmask;
+    }
+    const uint32_t cnt = min(ctl->q_blk, P.qcap), cur = ctl->cur;
     for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < cnt; e += gridDim.x * blockDim.x) {
         const uint2 q = queue[e];
         const bool kept = q.x < P.rows;
@@ -694,7 +760,15 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_sprt(ArrsacCtl *ctl, Arrsac
                                                            uint32_t *__restrict__ vm, uint32_t *__restrict__ pass_id,
                                                            uint32_t *__restrict__ pass_inl, cvb_pose *tposes, uint32_t *tinl,
                                                            uint32_t *tmasks) {
+    const uint32_t pb = blockIdx.x;
+    ctl += pb;
     if (ctl->done) return;
+    {
+        const ArsStrides S = ars_strides(P);
+        a += pb * S.a; b += pb * S.b; poses0 += pb * S.models0; nposes0 += pb * S.nposes0; masks0 += pb * S.models0 * P.W0;
+        vm += pb * S.vm; pass_id += pb * S.models0; pass_inl += pb * S.models0; tposes += pb * S.rows2; tinl += pb * S.rows2;
+        tmasks += pb * S.tmasks;
+    }
     __shared__ uint32_t sm[96], tot[3];
     extern __shared__ __align__(16) unsigned char ars_dyn[];     // 8 * ARS_SORT_CAP bytes
     uint64_t *keys = (uint64_t *)ars_dyn;                        // [ARS_SORT_CAP]
@@ -915,10 +989,24 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_book(ArrsacCtl *ctl, Arrsac
                                                            const cvb_pose *__restrict__ newposes, const uint8_t *__restrict__ nposes_new,
                                                            const uint32_t *__restrict__ newmask, uint32_t *__restrict__ pool,
                                                            uint32_t *__restrict__ samples_new, uint32_t *__restrict__ nout,
-                                                           unsigned long long loop_cond) {
+                                                           uint32_t *live, unsigned long long loop_cond) {
     // loop_cond: the handle of the graph's WHILE node when the block loop is a device-side loop (0 = unrolled launches);
-    // the node re-runs its body while the value is non-zero, so the loop's end is the one thing this kernel has to report
-    if (ctl->done) { if (loop_cond && threadIdx.x == 0) cudaGraphSetConditional(loop_cond, 0); return; }
+    // the node re-runs its body while the value is non-zero.  *live counts the problems of the batch still in the loop: the CTA
+    // that retires a finished problem decrements it, and the one that takes it to zero -- only that one -- ends the loop.
+    const uint32_t pb = blockIdx.x;
+    ctl += pb;
+    auto retire = [&]() {                                        // thread 0, once per problem
+        if (ctl->retired) return;
+        ctl->retired = 1;
+        if (atomicSub(live, 1u) == 1u && loop_cond) cudaGraphSetConditional(loop_cond, 0);
+    };
+    if (ctl->done) { if (threadIdx.x == 0) retire(); return; }
+    {
+        const ArsStrides S = ars_strides(P);
+        raw += (size_t)pb * P.nraw; tposes += pb * S.rows2; tinl += pb * S.rows2; tmasks += pb * S.tmasks; newposes += pb * S.nnew;
+        nposes_new += pb * S.nposes_new; newmask += pb * S.newmask; pool += (size_t)pb * P.NMAX; samples_new += pb * S.samples_new;
+        nout += pb * S.nnew;
+    }
     __shared__ __align__(8) uint32_t sm[96];
     __shared__ uint32_t tot[3];
     extern __shared__ __align__(16) unsigned char ars_dyn[];     // ARS_BOOK_SMEM bytes
@@ -965,7 +1053,7 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_book(ArrsacCtl *ctl, Arrsac
                 const uint32_t src = e_src[(uint32_t)keys[0] & 0xffffu];
                 ctl->winner = src < P.rows ? tp[src] : newposes[src - P.rows];
             }
-            if (loop_cond) cudaGraphSetConditional(loop_cond, 0);
+            retire();
         }
         return;
     }
@@ -1048,6 +1136,15 @@ __global__ void __launch_bounds__(ARS_BOOK_NT) k_ars_final(ArrsacCtl *ctl, Arrsa
                                                             const double *__restrict__ b, cvb_pose *model_out, uint32_t *inliers_out,
                                                             uint32_t cap, uint32_t *n_inliers_out, int32_t *found_out) {
     __shared__ uint32_t sm[96], tot[3];
+    const uint32_t pb = blockIdx.x;
+    {
+        const ArsStrides S = ars_strides(P);
+        ctl += pb; a += pb * S.a; b += pb * S.b;
+        if (model_out) model_out += pb;
+        if (inliers_out) inliers_out += (size_t)pb * cap;
+        if (n_inliers_out) n_inliers_out += pb;
+        if (found_out) found_out += pb;
+    }
     const uint32_t tid = threadIdx.x, NT = blockDim.x;
     const uint32_t n = ctl->n;
     const bool found = ctl->found != 0;

@@ -16,6 +16,7 @@
 #include "../../include/cvb200_tri.h"
 #include "../../include/cvb200_opt.h"
 #include "../../include/cvb200_pinhole.h"
+#include "../../include/cvb200_batch.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1630,18 +1631,20 @@ struct DevBuf {
 struct ArsWorkspace {
     DevBuf ctl, raw, samples0, poses0, nposes0, masks0, vm, pass_id, pass_inl, tposes, tinl, tmasks, newposes, nposes_new, newmask,
         nout, pool, samples_new, res, queue;
-    uint32_t *h_raw = nullptr;      // page-locked: raw draws + ArrsacCtl header
+    DevBuf bdata_a, bdata_b, bcounts;   // the host batch entry's padded rows and counts
+    uint32_t *h_raw = nullptr;      // page-locked: B ArrsacCtl headers + batch header, then B raw-draw streams
     size_t h_raw_cap = 0;
-    unsigned char *h_res = nullptr; // page-locked result block
+    unsigned char *h_res = nullptr; // page-locked result block (B ArrsacCtl)
+    size_t h_res_cap = 0;
     cudaEvent_t up_done = nullptr;  // the staging buffer may be rewritten once this has fired
-    std::vector<cvb_rng> snaps;     // generator state every ARS_SNAP draws of the staged stream
-    cvb_rng rng0;                   // generator state at draw 0 of the staged stream
-    uint32_t nraw = 0;
+    std::vector<cvb_rng> snaps;     // generator state every ARS_SNAP draws of each problem's staged stream (nsnap per problem)
+    uint32_t nraw = 0, nsnap = 0, B = 0;
     bool pending = false;           // a run whose draw count has not been committed to the caller's generator yet
+    bool pending_batch = false;     // ... and it came through the batch entry (committed by cvb_arrsac_commit_rng_batch only)
     // CUDA graphs of the whole run (two copies, ~20 + 3 per data block kernels, one copy back), keyed by everything the enqueue
     // depends on; a key is captured the second time it is seen (a one-off call does not pay the instantiation)
     struct GraphKey {
-        ArrsacParams P; int kind, row0; const void *a, *b, *n_dev; uint32_t n_host, nmax, cap, nb; const void *model, *inl, *ninl, *found;
+        ArrsacParams P; int kind, row0; const void *a, *b, *n_dev; uint32_t n_host, nmax, cap, nb, B; const void *model, *inl, *ninl, *found;
         const void *ws[22];
     };
     struct GraphEntry { GraphKey key; cudaGraphExec_t exec; uint64_t launches; uint32_t body; };   // body: launches of one WHILE body (0: no WHILE node)
@@ -1665,7 +1668,8 @@ void geom_workspace_free(GeomWorkspace *g) {
     if (g->ars) {
         ArsWorkspace *w = g->ars;
         DevBuf *ab[] = {&w->ctl, &w->raw, &w->samples0, &w->poses0, &w->nposes0, &w->masks0, &w->vm, &w->pass_id, &w->pass_inl, &w->tposes,
-                        &w->tinl, &w->tmasks, &w->newposes, &w->nposes_new, &w->newmask, &w->pool, &w->samples_new, &w->res, &w->queue};
+                        &w->tinl, &w->tmasks, &w->newposes, &w->nposes_new, &w->newmask, &w->nout, &w->pool, &w->samples_new, &w->res,
+                        &w->queue, &w->bdata_a, &w->bdata_b, &w->bcounts};
         for (DevBuf *d : ab) if (d->p) cudaFree(d->p);
         if (w->h_raw) cudaFreeHost(w->h_raw);
         if (w->h_res) cudaFreeHost(w->h_res);
@@ -1914,9 +1918,13 @@ ArsWorkspace *arsws(cvb_ctx *ctx) {
     return g->ars;
 }
 
-int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const double *a_dev, const double *b_dev, const uint32_t *n_dev,
-                   uint32_t n_host, uint32_t nmax, const cvb_rng *rng, cvb_pose *model_dev, uint32_t *inl_dev, uint32_t cap,
-                   uint32_t *ninl_dev, int32_t *found_dev, int row0) {
+// B independent problems in one set of launches (arrsac_dev.cuh: problem pb = blockIdx.x of the one-CTA kernels, blockIdx.y of the
+// grids).  Problem pb reads rows [pb * nmax, pb * nmax + min(n, nmax)) of a_dev / b_dev with n = n_dev[pb] (n_host when n_dev is
+// NULL), draws from its own generator rngs[pb] and writes model_dev[pb], inl_dev[pb * cap ..], ninl_dev[pb], found_dev[pb].
+// `batch` records which commit entry owns the run (B = 1 through the single entry is that entry's run, launch for launch).
+int arrsac_run_dev_batch(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const double *a_dev, const double *b_dev, const uint32_t *n_dev,
+                         uint32_t n_host, uint32_t nmax, uint32_t B, const cvb_rng *rngs, cvb_pose *model_dev, uint32_t *inl_dev, uint32_t cap,
+                         uint32_t *ninl_dev, int32_t *found_dev, int row0, bool batch) {
     if (cfg->block_size == 0 || cfg->initialization_blocks == 0) return cvb_set_error(ctx, CVB_EINVAL, "block_size / initialization_blocks must be > 0");
     ArrsacParams P;
     memset(&P, 0, sizeof(P));
@@ -1941,51 +1949,61 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     ArsWorkspace *w = arsws(ctx);
     const uint32_t nb_max = cdiv(P.NMAX, P.bs) + 1;
     const uint32_t nraw = P.H0 * P.K + P.H0 * P.K / 4 + 64 + nb_max * (P.G * P.K + P.G * P.K / 4 + 64);
-    const size_t nmodels0 = (size_t)P.H0 * P.MM, nnew = (size_t)std::max<uint32_t>(P.G, 1) * P.MM;
+    P.nraw = nraw; P.qcap = ARS_QCAP / B; P.sdata = nmax;
+    const ArsStrides S = ars_strides(P);
     int rc;
-    if ((rc = w->ctl.ensure(ctx, sizeof(ArrsacCtl)))) return rc;
-    if ((rc = w->raw.ensure(ctx, sizeof(uint32_t) * (size_t)nraw))) return rc;
-    if ((rc = w->samples0.ensure(ctx, sizeof(uint32_t) * (size_t)std::max<uint32_t>(P.H0, 1) * P.K))) return rc;
-    if ((rc = w->poses0.ensure(ctx, sizeof(cvb_pose) * std::max<size_t>(nmodels0, 1)))) return rc;
-    if ((rc = w->nposes0.ensure(ctx, std::max<uint32_t>(P.H0, 1)))) return rc;
-    if ((rc = w->masks0.ensure(ctx, sizeof(uint32_t) * std::max<size_t>(nmodels0, 1) * P.W0))) return rc;
-    if ((rc = w->vm.ensure(ctx, sizeof(uint32_t) * std::max<size_t>(nmodels0, ARS_SORT_CAP)))) return rc;
-    if ((rc = w->pass_id.ensure(ctx, sizeof(uint32_t) * std::max<size_t>(nmodels0, 1)))) return rc;
-    if ((rc = w->pass_inl.ensure(ctx, sizeof(uint32_t) * std::max<size_t>(nmodels0, 1)))) return rc;
-    if ((rc = w->tposes.ensure(ctx, sizeof(cvb_pose) * 2 * (size_t)P.rows))) return rc;
-    if ((rc = w->tinl.ensure(ctx, sizeof(uint32_t) * 2 * (size_t)P.rows))) return rc;
-    if ((rc = w->tmasks.ensure(ctx, sizeof(uint32_t) * 2 * (size_t)P.rows * P.NW))) return rc;
-    if ((rc = w->newposes.ensure(ctx, sizeof(cvb_pose) * nnew))) return rc;
-    if ((rc = w->nposes_new.ensure(ctx, std::max<uint32_t>(P.G, 1)))) return rc;
-    if ((rc = w->newmask.ensure(ctx, sizeof(uint32_t) * nnew * P.NW))) return rc;
-    if ((rc = w->nout.ensure(ctx, sizeof(uint32_t) * nnew))) return rc;
-    if ((rc = w->pool.ensure(ctx, sizeof(uint32_t) * (size_t)P.NMAX))) return rc;
-    if ((rc = w->samples_new.ensure(ctx, sizeof(uint32_t) * (size_t)std::max<uint32_t>(P.G, 1) * P.K))) return rc;
+    // B slices of every buffer (ars_strides); the queue keeps its size, split between the problems
+    if ((rc = w->ctl.ensure(ctx, sizeof(ArrsacCtl) * B + 16))) return rc;
+    if ((rc = w->raw.ensure(ctx, sizeof(uint32_t) * (size_t)nraw * B))) return rc;
+    if ((rc = w->samples0.ensure(ctx, sizeof(uint32_t) * S.samples0 * B))) return rc;
+    if ((rc = w->poses0.ensure(ctx, sizeof(cvb_pose) * S.models0 * B))) return rc;
+    if ((rc = w->nposes0.ensure(ctx, S.nposes0 * B))) return rc;
+    if ((rc = w->masks0.ensure(ctx, sizeof(uint32_t) * S.models0 * P.W0 * B))) return rc;
+    if ((rc = w->vm.ensure(ctx, sizeof(uint32_t) * S.vm * B))) return rc;
+    if ((rc = w->pass_id.ensure(ctx, sizeof(uint32_t) * S.models0 * B))) return rc;
+    if ((rc = w->pass_inl.ensure(ctx, sizeof(uint32_t) * S.models0 * B))) return rc;
+    if ((rc = w->tposes.ensure(ctx, sizeof(cvb_pose) * S.rows2 * B))) return rc;
+    if ((rc = w->tinl.ensure(ctx, sizeof(uint32_t) * S.rows2 * B))) return rc;
+    if ((rc = w->tmasks.ensure(ctx, sizeof(uint32_t) * S.tmasks * B))) return rc;
+    if ((rc = w->newposes.ensure(ctx, sizeof(cvb_pose) * S.nnew * B))) return rc;
+    if ((rc = w->nposes_new.ensure(ctx, S.nposes_new * B))) return rc;
+    if ((rc = w->newmask.ensure(ctx, sizeof(uint32_t) * S.newmask * B))) return rc;
+    if ((rc = w->nout.ensure(ctx, sizeof(uint32_t) * S.nnew * B))) return rc;
+    if ((rc = w->pool.ensure(ctx, sizeof(uint32_t) * (size_t)P.NMAX * B))) return rc;
+    if ((rc = w->samples_new.ensure(ctx, sizeof(uint32_t) * S.samples_new * B))) return rc;
     if ((rc = w->queue.ensure(ctx, sizeof(uint2) * 2 * (size_t)ARS_QCAP))) return rc;
-    // page-locked staging: [ArrsacCtl header | raw draws]
-    const size_t hdr = (sizeof(ArrsacCtl) + 15) / 16 * 16, stage_bytes = hdr + sizeof(uint32_t) * (size_t)nraw;
+    // page-locked staging: [B ArrsacCtl headers | batch header (live count) | B raw-draw streams]
+    const size_t ctl_bytes = sizeof(ArrsacCtl) * B + 16;
+    const size_t hdr = (ctl_bytes + 15) / 16 * 16, stage_bytes = hdr + sizeof(uint32_t) * (size_t)nraw * B;
     if (w->h_raw_cap < stage_bytes) {
         if (w->h_raw) { cvb_wait(ctx, ctx->stream); cudaFreeHost(w->h_raw); w->h_raw = nullptr; w->h_raw_cap = 0; }
         if (cudaHostAlloc((void **)&w->h_raw, stage_bytes, cudaHostAllocDefault) != cudaSuccess) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked staging");
         w->h_raw_cap = stage_bytes;
     }
-    if (!w->h_res && cudaHostAlloc((void **)&w->h_res, sizeof(ArrsacCtl) + sizeof(cvb_pose) + 64, cudaHostAllocDefault) != cudaSuccess)
-        return cvb_set_error(ctx, CVB_ENOMEM, "page-locked staging");
+    const size_t res_bytes = sizeof(ArrsacCtl) * B + sizeof(cvb_pose) + 64;
+    if (w->h_res_cap < res_bytes) {
+        if (w->h_res) { cvb_wait(ctx, ctx->stream); cudaFreeHost(w->h_res); w->h_res = nullptr; w->h_res_cap = 0; }
+        if (cudaHostAlloc((void **)&w->h_res, res_bytes, cudaHostAllocDefault) != cudaSuccess) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked staging");
+        w->h_res_cap = res_bytes;
+    }
     if (!w->up_done) CVB_CUDA(ctx, cudaEventCreateWithFlags(&w->up_done, cudaEventDisableTiming | cudaEventBlockingSync));
     else CVB_CUDA(ctx, cudaEventSynchronize(w->up_done));       // previous upload has left the staging buffer
     {
-        cvb_rng g = *rng;
-        w->rng0 = g;
-        w->snaps.clear();
-        uint32_t *raw = (uint32_t *)((unsigned char *)w->h_raw + hdr);
-        for (uint32_t i = 0; i < nraw; i++) {
-            if (i % ARS_SNAP == 0) w->snaps.push_back(g);
-            raw[i] = cvb_rng_next_u32(&g);
+        w->nsnap = cdiv(nraw, ARS_SNAP);
+        w->snaps.resize((size_t)w->nsnap * B);
+        memset(w->h_raw, 0, hdr);
+        for (uint32_t pb = 0; pb < B; pb++) {
+            cvb_rng g = rngs[pb];
+            uint32_t *raw = (uint32_t *)((unsigned char *)w->h_raw + hdr) + (size_t)pb * nraw;
+            for (uint32_t i = 0; i < nraw; i++) {
+                if (i % ARS_SNAP == 0) w->snaps[(size_t)pb * w->nsnap + i / ARS_SNAP] = g;
+                raw[i] = cvb_rng_next_u32(&g);
+            }
+            ArrsacCtl *h = (ArrsacCtl *)w->h_raw + pb;
+            h->nraw = nraw; h->gen = g; h->gen_pos = nraw; h->rng_pos = 0;
         }
-        ArrsacCtl *h = (ArrsacCtl *)w->h_raw;
-        memset(h, 0, sizeof(*h));
-        h->nraw = nraw; h->gen = g; h->gen_pos = nraw; h->rng_pos = 0;
-        w->nraw = nraw;
+        *(uint32_t *)((unsigned char *)w->h_raw + sizeof(ArrsacCtl) * B) = B;     // live problems
+        w->nraw = nraw; w->B = B;
     }
     cudaStream_t st = ctx->stream;
     static bool attr_set = false;
@@ -2001,15 +2019,16 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     uint32_t body_launches = 0;
     // everything the stream sees, from the upload of the draw stream to the copy of the control block back
     auto enqueue = [&]() -> int {
-        CVB_CUDA(ctx, cudaMemcpyAsync(w->ctl.p, w->h_raw, sizeof(ArrsacCtl), cudaMemcpyHostToDevice, st));
-        CVB_CUDA(ctx, cudaMemcpyAsync(w->raw.p, (unsigned char *)w->h_raw + hdr, sizeof(uint32_t) * (size_t)nraw, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(w->ctl.p, w->h_raw, ctl_bytes, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(w->raw.p, (unsigned char *)w->h_raw + hdr, sizeof(uint32_t) * (size_t)nraw * B, cudaMemcpyHostToDevice, st));
         if (!capturing) CVB_CUDA(ctx, cudaEventRecord(w->up_done, st));      // eager: the staging buffer is free as soon as the two copies are done
         ArrsacCtl *ctl = (ArrsacCtl *)w->ctl.p;
+        uint32_t *live = (uint32_t *)((unsigned char *)w->ctl.p + sizeof(ArrsacCtl) * B);
         const uint32_t *raw = (const uint32_t *)w->raw.p;
         const int res = kind_res(kind);
         {
             CVB_PROF(ctx, "k_ars_begin", 0);
-            k_ars_begin<<<1, ARS_BOOK_NT, 0, st>>>(ctl, P, n_dev, n_host, raw, (uint32_t *)w->samples0.p);
+            k_ars_begin<<<B, ARS_BOOK_NT, 0, st>>>(ctl, P, n_dev, n_host, raw, (uint32_t *)w->samples0.p);
             CVB_LAUNCH_CHECK(ctx);
         }
         auto estimate = [&](int phase, uint32_t H, const uint32_t *samples, cvb_pose *poses, uint8_t *nposes) -> int {
@@ -2018,10 +2037,10 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             // the big initial batch is bound by FP64 issue (4 lanes per hypothesis waste the fewest slots); a block's 64 hypotheses
             // are a latency chain in front of the next scoring (16 lanes: the shortest chain)
             // (8 lanes, or 16 lanes at 64 registers, measured the same 0.137-0.140 ms for the initial batch)
-            if (kind == 0 && phase == 0) k_ars_estimate8<4, 5><<<cdiv(H, 128 / 4), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes);
-            else if (kind == 0) k_ars_estimate8<16, 5><<<cdiv(H, 128 / 16), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes);
-            else if (kind == 1) k_ars_estimate<1><<<cdiv(H, 128), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, row0);
-            else k_ars_estimate<2><<<cdiv(H, 128), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, row0);
+            if (kind == 0 && phase == 0) k_ars_estimate8<4, 5><<<dim3(cdiv(H, 128 / 4), B), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, P);
+            else if (kind == 0) k_ars_estimate8<16, 5><<<dim3(cdiv(H, 128 / 16), B), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, P);
+            else if (kind == 1) k_ars_estimate<1><<<dim3(cdiv(H, 128), B), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, row0, P);
+            else k_ars_estimate<2><<<dim3(cdiv(H, 128), B), 128, 0, st>>>(ctl, phase, H, a_dev, b_dev, samples, poses, nposes, row0, P);
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
@@ -2043,12 +2062,12 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             const uint32_t sgrid = phase == 1 ? sgrid_block : sgrid_full;
             CVB_PROF(ctx, phase == 1 ? "k_ars_score_block" : "k_ars_score_init", 0);
             if (res == 0)
-                k_ars_score<0><<<sgrid, 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
+                k_ars_score<0><<<dim3(sgrid, B), 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
                                                       (uint32_t *)w->masks0.p, (const cvb_pose *)w->tposes.p, (uint32_t *)w->tmasks.p,
                                                       (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p,
                                                       (uint32_t *)w->nout.p);
             else
-                k_ars_score<1><<<sgrid, 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
+                k_ars_score<1><<<dim3(sgrid, B), 256, score_smem, st>>>(ctl, (uint2 *)w->queue.p, P, phase, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p,
                                                       (uint32_t *)w->masks0.p, (const cvb_pose *)w->tposes.p, (uint32_t *)w->tmasks.p,
                                                       (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p, (uint32_t *)w->newmask.p,
                                                       (uint32_t *)w->nout.p);
@@ -2058,7 +2077,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         if ((rc = estimate(0, P.H0, (const uint32_t *)w->samples0.p, (cvb_pose *)w->poses0.p, (uint8_t *)w->nposes0.p))) return rc;
         auto resolve = [&](int stage) -> int {
             CVB_PROF(ctx, "k_ars_resolve", 0);
-            k_ars_resolve<<<sgrid_full, 256, 0, st>>>(ctl, (const uint2 *)w->queue.p, stage, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (uint32_t *)w->masks0.p);
+            k_ars_resolve<<<dim3(sgrid_full, B), 256, 0, st>>>(ctl, (const uint2 *)w->queue.p, stage, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (uint32_t *)w->masks0.p);
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
@@ -2071,11 +2090,11 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         {
             CVB_PROF(ctx, "k_ars_sprt", 0);
             if (res == 0)
-                k_ars_sprt<0><<<1, ARS_BOOK_NT, 8 * ARS_SORT_CAP, st>>>(ctl, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p, (uint32_t *)w->masks0.p,
+                k_ars_sprt<0><<<B, ARS_BOOK_NT, 8 * ARS_SORT_CAP, st>>>(ctl, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p, (uint32_t *)w->masks0.p,
                                                         (uint32_t *)w->vm.p, (uint32_t *)w->pass_id.p, (uint32_t *)w->pass_inl.p, (cvb_pose *)w->tposes.p,
                                                         (uint32_t *)w->tinl.p, (uint32_t *)w->tmasks.p);
             else
-                k_ars_sprt<1><<<1, ARS_BOOK_NT, 8 * ARS_SORT_CAP, st>>>(ctl, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p, (uint32_t *)w->masks0.p,
+                k_ars_sprt<1><<<B, ARS_BOOK_NT, 8 * ARS_SORT_CAP, st>>>(ctl, P, a_dev, b_dev, (const cvb_pose *)w->poses0.p, (const uint8_t *)w->nposes0.p, (uint32_t *)w->masks0.p,
                                                         (uint32_t *)w->vm.p, (uint32_t *)w->pass_id.p, (uint32_t *)w->pass_inl.p, (cvb_pose *)w->tposes.p,
                                                         (uint32_t *)w->tinl.p, (uint32_t *)w->tmasks.p);
             CVB_LAUNCH_CHECK(ctx);
@@ -2087,10 +2106,10 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         const uint32_t nb = n_bound > init_n ? cdiv(n_bound - init_n, P.bs) : 0;
         auto book = [&](unsigned long long cond) -> int {
             CVB_PROF(ctx, "k_ars_book", 0);
-            k_ars_book<<<1, ARS_BOOK_NT, ARS_BOOK_SMEM, st>>>(ctl, P, raw, (cvb_pose *)w->tposes.p, (uint32_t *)w->tinl.p, (uint32_t *)w->tmasks.p,
+            k_ars_book<<<B, ARS_BOOK_NT, ARS_BOOK_SMEM, st>>>(ctl, P, raw, (cvb_pose *)w->tposes.p, (uint32_t *)w->tinl.p, (uint32_t *)w->tmasks.p,
                                                               (const cvb_pose *)w->newposes.p, (const uint8_t *)w->nposes_new.p,
                                                               (const uint32_t *)w->newmask.p, (uint32_t *)w->pool.p, (uint32_t *)w->samples_new.p,
-                                                              (uint32_t *)w->nout.p, cond);
+                                                              (uint32_t *)w->nout.p, live, cond);
             CVB_LAUNCH_CHECK(ctx);
             return 0;
         };
@@ -2100,7 +2119,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             if (res == 0) {
                 CVB_PROF(ctx, "k_ars_resolve_block", 0);
                 // 64-thread CTAs: a block queues a small fraction of its predicates, spread over as many SMs as possible
-                k_ars_resolve_block<<<sgrid_full, 64, 0, st>>>(ctl, (const uint2 *)w->queue.p, P, a_dev, b_dev, (const cvb_pose *)w->tposes.p,
+                k_ars_resolve_block<<<dim3(sgrid_full, B), 64, 0, st>>>(ctl, (const uint2 *)w->queue.p, P, a_dev, b_dev, (const cvb_pose *)w->tposes.p,
                                                                (uint32_t *)w->tmasks.p, (const cvb_pose *)w->newposes.p, (uint32_t *)w->newmask.p);
                 CVB_LAUNCH_CHECK(ctx);
             }
@@ -2143,11 +2162,11 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         }
         {
             CVB_PROF(ctx, "k_ars_final", 0);
-            if (res == 0) k_ars_final<0><<<1, ARS_BOOK_NT, 0, st>>>(ctl, P, a_dev, b_dev, model_dev, inl_dev, cap, ninl_dev, found_dev);
-            else k_ars_final<1><<<1, ARS_BOOK_NT, 0, st>>>(ctl, P, a_dev, b_dev, model_dev, inl_dev, cap, ninl_dev, found_dev);
+            if (res == 0) k_ars_final<0><<<B, ARS_BOOK_NT, 0, st>>>(ctl, P, a_dev, b_dev, model_dev, inl_dev, cap, ninl_dev, found_dev);
+            else k_ars_final<1><<<B, ARS_BOOK_NT, 0, st>>>(ctl, P, a_dev, b_dev, model_dev, inl_dev, cap, ninl_dev, found_dev);
             CVB_LAUNCH_CHECK(ctx);
         }
-        CVB_CUDA(ctx, cudaMemcpyAsync(w->h_res, w->ctl.p, sizeof(ArrsacCtl), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(w->h_res, w->ctl.p, sizeof(ArrsacCtl) * B, cudaMemcpyDeviceToHost, st));
         return 0;
     };
     if (w->use_graph < 0) {
@@ -2156,12 +2175,12 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     }
     if (!w->use_graph || ctx->prof) {
         if ((rc = enqueue())) return rc;
-        w->pending = true;
+        w->pending = true; w->pending_batch = batch;
         return 0;
     }
     ArsWorkspace::GraphKey key;
     memset(&key, 0, sizeof(key));
-    key.P = P; key.kind = kind; key.row0 = row0; key.a = a_dev; key.b = b_dev; key.n_dev = n_dev; key.n_host = n_host; key.nmax = nmax; key.cap = cap;
+    key.P = P; key.kind = kind; key.row0 = row0; key.a = a_dev; key.b = b_dev; key.n_dev = n_dev; key.n_host = n_host; key.nmax = nmax; key.cap = cap; key.B = B;
     key.model = model_dev; key.inl = inl_dev; key.ninl = ninl_dev; key.found = found_dev;
     {
         const DevBuf *bufs[] = {&w->ctl, &w->raw, &w->samples0, &w->poses0, &w->nposes0, &w->masks0, &w->vm, &w->pass_id, &w->pass_inl, &w->tposes,
@@ -2177,7 +2196,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
             CVB_CUDA(ctx, cudaEventRecord(w->up_done, st));       // replay: the staging buffer is free when the run is over
             ctx->launches += ge.launches;
             w->last_body = ge.body;
-            w->pending = true;
+            w->pending = true; w->pending_batch = batch;
             return 0;
         }
     bool seen = false;
@@ -2186,7 +2205,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         if (w->seen.size() >= 64) w->seen.erase(w->seen.begin());
         w->seen.push_back(key);
         if ((rc = enqueue())) return rc;
-        w->pending = true;
+        w->pending = true; w->pending_batch = batch;
         return 0;
     }
     const uint64_t l0 = ctx->launches;
@@ -2222,7 +2241,7 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
         w->use_graph = 0;
         ctx->launches = l0;
         if ((rc = enqueue())) return rc;
-        w->pending = true;
+        w->pending = true; w->pending_batch = batch;
         return 0;
     }
     if (w->graphs.size() >= 16) { cudaGraphExecDestroy(w->graphs.front().exec); w->graphs.erase(w->graphs.begin()); }
@@ -2230,37 +2249,69 @@ int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const doub
     w->last_body = while_loop ? body_launches : 0u;
     CVB_CUDA(ctx, cudaGraphLaunch(exec, st));
     CVB_CUDA(ctx, cudaEventRecord(w->up_done, st));
-    w->pending = true;
+    w->pending = true; w->pending_batch = batch;
     return 0;
 }
 
+int arrsac_run_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, const double *a_dev, const double *b_dev, const uint32_t *n_dev,
+                   uint32_t n_host, uint32_t nmax, const cvb_rng *rng, cvb_pose *model_dev, uint32_t *inl_dev, uint32_t cap,
+                   uint32_t *ninl_dev, int32_t *found_dev, int row0) {
+    return arrsac_run_dev_batch(ctx, cfg, kind, a_dev, b_dev, n_dev, n_host, nmax, 1, rng, model_dev, inl_dev, cap, ninl_dev, found_dev, row0, false);
+}
+
 // after the stream has drained: advance the caller's generator by the draws the run consumed (state in == state the
-// reference would hold after model_inliers)
-int arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, ArrsacCtl *stats_out = nullptr) {
+// reference would hold after model_inliers).  rngs / stats_out: one per problem of the pending run (B of them); `batch` must match
+// the entry that started the run, so a run is never committed as the other kind.
+int arrsac_commit_rng_batch(cvb_ctx *ctx, cvb_rng *rngs, uint32_t B, ArrsacCtl *stats_out, bool batch) {
     ArsWorkspace *w = arsws(ctx);
     if (!w->pending) return cvb_set_error(ctx, CVB_EINVAL, "no device ARRSAC run to commit");
-    const ArrsacCtl *h = (const ArrsacCtl *)w->h_res;
-    if (stats_out) *stats_out = *h;
+    if (w->pending_batch != batch)
+        return cvb_set_error(ctx, CVB_EINVAL, batch ? "the pending ARRSAC run is a single run: commit it with cvb_arrsac_commit_rng"
+                                                    : "the pending ARRSAC run is a batch: commit it with cvb_arrsac_commit_rng_batch");
+    if (B != w->B) return cvb_set_error(ctx, CVB_EINVAL, "the pending ARRSAC run has %u problems, not %u", w->B, B);
+    const ArrsacCtl *hs = (const ArrsacCtl *)w->h_res;
+    if (stats_out) memcpy(stats_out, hs, sizeof(ArrsacCtl) * B);
     if (getenv("CVB_ARS_DEBUG"))
-        fprintf(stderr, "[arrsac] n %u models %u pass %u chunks %u turns %u repairs %u lazy %u | sprt us: order %u walk %u commit %u | block iterations %u"
-                " | undecided predicates queued: initial %u block %u | block units: kept %u new %u skipped %u | blocks worst0 %u bar<32 %u not estimated %u\n",
-                h->n, h->Mv, h->npass, h->stat_chunks, h->stat_turns, h->stat_repairs, h->stat_lazy, h->stat_perm_us, h->stat_walk_us,
-                h->stat_commit_us, h->iters, h->q_count + h->q_count2, h->stat_qblk, h->stat_units_kept, h->stat_units_new, h->stat_skip,
-                h->stat_blk_w0, h->stat_blk_lt32, h->stat_blk_bar0);
-    ctx->launches += (uint64_t)w->last_body * h->iters;          // the WHILE body ran iters + 1 times, the capture counted it once
+        for (uint32_t pb = 0; pb < B; pb++) {
+            const ArrsacCtl *h = hs + pb;
+            fprintf(stderr, "[arrsac] n %u models %u pass %u chunks %u turns %u repairs %u lazy %u | sprt us: order %u walk %u commit %u | block iterations %u"
+                    " | undecided predicates queued: initial %u block %u | block units: kept %u new %u skipped %u | blocks worst0 %u bar<32 %u not estimated %u\n",
+                    h->n, h->Mv, h->npass, h->stat_chunks, h->stat_turns, h->stat_repairs, h->stat_lazy, h->stat_perm_us, h->stat_walk_us,
+                    h->stat_commit_us, h->iters, h->q_count + h->q_count2, h->stat_qblk, h->stat_units_kept, h->stat_units_new, h->stat_skip,
+                    h->stat_blk_w0, h->stat_blk_lt32, h->stat_blk_bar0);
+        }
+    // the WHILE body ran (most block iterations of any problem) + 1 times, the capture counted it once
+    uint32_t iters = 0;
+    for (uint32_t pb = 0; pb < B; pb++) iters = std::max(iters, hs[pb].iters);
+    ctx->launches += (uint64_t)w->last_body * iters;
     w->last_body = 0;
     w->pending = false;
-    if (!rng) return 0;
-    const uint64_t used = h->rng_pos;
-    if (used >= w->nraw) {
-        if (h->gen_pos != std::max<uint64_t>(used, w->nraw)) return cvb_set_error(ctx, CVB_ECUDA, "generator position mismatch");
-        *rng = h->gen;
-        return 0;
+    if (!rngs) return 0;
+    // every problem is checked before any generator is written: an error leaves all of them where they were
+    for (uint32_t pb = 0; pb < B; pb++)
+        if (hs[pb].rng_pos >= w->nraw && hs[pb].gen_pos != std::max<uint64_t>(hs[pb].rng_pos, w->nraw))
+            return cvb_set_error(ctx, CVB_ECUDA, "generator position mismatch (problem %u)", pb);
+    for (uint32_t pb = 0; pb < B; pb++) {
+        const uint64_t used = hs[pb].rng_pos;
+        if (used >= w->nraw) { rngs[pb] = hs[pb].gen; continue; }
+        cvb_rng g = w->snaps[(size_t)pb * w->nsnap + used / ARS_SNAP];
+        for (uint64_t i = used / ARS_SNAP * ARS_SNAP; i < used; i++) cvb_rng_next_u32(&g);
+        rngs[pb] = g;
     }
-    cvb_rng g = w->snaps[used / ARS_SNAP];
-    for (uint64_t i = used / ARS_SNAP * ARS_SNAP; i < used; i++) cvb_rng_next_u32(&g);
-    *rng = g;
     return 0;
+}
+// the 16 statistics words of cvb_arrsac_commit_rng (13..15 reserved): n, valid initial models, SPRT passes, SPRT commit rounds, block
+// iterations, draws, inliers, found, 32-datum units scored in stage 1 / stage 2, predicates resolved exactly from the queues, mask
+// words computed by the SPRT itself, SPRT repairs
+void arrsac_stats_words(const ArrsacCtl &h, uint32_t *o) {
+    o[0] = h.n; o[1] = h.Mv; o[2] = h.npass; o[3] = h.stat_chunks; o[4] = h.iters;
+    o[5] = (uint32_t)h.rng_pos; o[6] = h.n_inliers; o[7] = h.found;
+    o[8] = h.stat_units0; o[9] = h.stat_units2; o[10] = h.q_count + h.q_count2; o[11] = h.stat_lazy;
+    o[12] = h.stat_repairs; o[13] = h.stat_pad /* data walked by the box walks */; o[14] = h.stat_walk_us; o[15] = h.stat_commit_us;
+}
+
+int arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, ArrsacCtl *stats_out = nullptr) {
+    return arrsac_commit_rng_batch(ctx, rng, 1, stats_out, false);
 }
 
 // host-pointer entry: upload, run on the device, one synchronisation at the end
@@ -2362,6 +2413,151 @@ int download_poses_updates(cvb_ctx *ctx, GeomWorkspace *g, cvb_pose *poses_out, 
 }
 
 }  // namespace
+
+// ---- batched device ARRSAC (C names in batch_abi.cu, include/cvb200_batch.h) ------------------------------------------------
+static int ars_batch_check(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, int row0, uint32_t B, const cvb_rng *rngs) {
+    if (B > CVB_ARRSAC_BATCH_MAX) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "batch of %u problems: at most %u", B, CVB_ARRSAC_BATCH_MAX);
+    if (!cfg || !rngs) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (kind < 0 || kind > 2) return cvb_set_error(ctx, CVB_EINVAL, "kind must be 0 (eight-point), 1 (P3P) or 2 (five-point)");
+    if (kind == 2 && row0 != 5 && row0 != 6) return cvb_set_error(ctx, CVB_EINVAL, "eigenvector_row0 must be 5 (reference) or 6 (corrected)");
+    return 0;
+}
+
+int ars_batch_dev(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, int row0, const double *a_dev, const double *b_dev, const uint32_t *n_dev,
+                  uint32_t n_max, uint32_t B, const cvb_rng *rngs, cvb_pose *model_out_dev, uint32_t *inliers_out_dev, uint32_t cap,
+                  uint32_t *n_inliers_dev, int32_t *found_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (B == 0) return 0;
+    int rc = ars_batch_check(ctx, cfg, kind, row0, B, rngs);
+    if (rc) return rc;
+    if (!a_dev || !b_dev || !model_out_dev || !n_inliers_dev || !found_dev) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    return arrsac_run_dev_batch(ctx, cfg, kind, a_dev, b_dev, n_dev, n_max, n_max, B, rngs, model_out_dev, inliers_out_dev, cap, n_inliers_dev,
+                                found_dev, kind == 2 ? row0 : 5, true);
+}
+
+int ars_commit_rng_batch(cvb_ctx *ctx, cvb_rng *rngs, uint32_t B, uint32_t *stats_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (!rngs) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    std::vector<ArrsacCtl> h(std::max<uint32_t>(B, 1));
+    int rc = arrsac_commit_rng_batch(ctx, rngs, B, h.data(), true);
+    if (rc) return rc;
+    if (stats_out)
+        for (uint32_t pb = 0; pb < B; pb++) arrsac_stats_words(h[pb], stats_out + 16 * (size_t)pb);
+    return 0;
+}
+
+int ars_batch_host(cvb_ctx *ctx, const cvb_arrsac_cfg *cfg, int kind, int row0, const double *a, const double *b, const uint32_t *offsets,
+                   uint32_t B, cvb_rng *rngs, cvb_pose *models_out, uint32_t *inliers_out, uint32_t *n_inliers_out, int32_t *found_out) {
+    if (!ctx) return CVB_EINVAL;
+    if (B == 0) return 0;
+    int rc = ars_batch_check(ctx, cfg, kind, row0, B, rngs);
+    if (rc) return rc;
+    if (!offsets || !models_out || !n_inliers_out || !found_out) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    uint32_t n_max = 0;
+    for (uint32_t pb = 0; pb < B; pb++) {
+        if (offsets[pb + 1] < offsets[pb]) return cvb_set_error(ctx, CVB_EINVAL, "offsets must be non-decreasing");
+        n_max = std::max(n_max, offsets[pb + 1] - offsets[pb]);
+    }
+    const uint32_t total = offsets[B] - offsets[0];
+    if (total && (!a || !b)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    for (uint32_t pb = 0; pb < B; pb++) { found_out[pb] = 0; n_inliers_out[pb] = 0; }
+    // every problem below MIN_SAMPLES: nothing runs and no generator moves (as in the single entries)
+    if (n_max < kind_K(kind) || cfg->initialization_hypotheses == 0) return 0;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    ArsWorkspace *w = arsws(ctx);
+    const uint32_t bc = kind_res(kind) == 0 ? 3 : 4;
+    {   // problem pb's rows at pb * n_max (padding rows are never read: the kernels stop at the problem's count)
+        std::vector<double> pa((size_t)B * n_max * 3, 0.0), pbv((size_t)B * n_max * bc, 0.0);
+        std::vector<uint32_t> cnt(B);
+        for (uint32_t pb = 0; pb < B; pb++) {
+            cnt[pb] = offsets[pb + 1] - offsets[pb];
+            if (!cnt[pb]) continue;
+            memcpy(pa.data() + (size_t)pb * n_max * 3, a + 3 * (size_t)offsets[pb], sizeof(double) * 3 * cnt[pb]);
+            memcpy(pbv.data() + (size_t)pb * n_max * bc, b + bc * (size_t)offsets[pb], sizeof(double) * bc * cnt[pb]);
+        }
+        if ((rc = upload(ctx, w->bdata_a, pa.data(), sizeof(double) * pa.size()))) return rc;
+        if ((rc = upload(ctx, w->bdata_b, pbv.data(), sizeof(double) * pbv.size()))) return rc;
+        if ((rc = upload(ctx, w->bcounts, cnt.data(), sizeof(uint32_t) * B))) return rc;
+        CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));       // the pageable sources leave scope
+    }
+    // result block: B poses | B counts | B found flags | B x n_max inlier indices
+    const size_t pose_b = sizeof(cvb_pose) * B, res_bytes = pose_b + 8 * (size_t)B + sizeof(uint32_t) * (size_t)B * n_max;
+    if ((rc = w->res.ensure(ctx, res_bytes))) return rc;
+    unsigned char *rd = (unsigned char *)w->res.p;
+    if ((rc = arrsac_run_dev_batch(ctx, cfg, kind, (const double *)w->bdata_a.p, (const double *)w->bdata_b.p, (const uint32_t *)w->bcounts.p,
+                                   n_max, n_max, B, rngs, (cvb_pose *)rd, (uint32_t *)(rd + pose_b + 8 * (size_t)B), n_max,
+                                   (uint32_t *)(rd + pose_b), (int32_t *)(rd + pose_b + 4 * (size_t)B), kind == 2 ? row0 : 5, true))) return rc;
+    unsigned char *hs = (unsigned char *)cvb_pinned(ctx, res_bytes);
+    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs, rd, res_bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    if ((rc = arrsac_commit_rng_batch(ctx, rngs, B, nullptr, true))) return rc;
+    const uint32_t *ninl = (const uint32_t *)(hs + pose_b);
+    const int32_t *fnd = (const int32_t *)(hs + pose_b + 4 * (size_t)B);
+    const uint32_t *inl = (const uint32_t *)(hs + pose_b + 8 * (size_t)B);
+    for (uint32_t pb = 0; pb < B; pb++) {
+        found_out[pb] = fnd[pb];
+        if (!fnd[pb]) continue;
+        memcpy(models_out + pb, hs + sizeof(cvb_pose) * pb, sizeof(cvb_pose));
+        n_inliers_out[pb] = ninl[pb];
+        if (inliers_out) memcpy(inliers_out + offsets[pb] - offsets[0], inl + (size_t)pb * n_max, sizeof(uint32_t) * ninl[pb]);
+    }
+    return 0;
+}
+
+// cv-sfm's init_two_view (cv-sfm/src/lib.rs:1365-1432) of frame `center` against F option frames, on the outputs of
+// cvb_frame_features_batch_dev: F symmetric matches, one gather of the matched bearings for all options, one batched ARRSAC.
+// Option f's consensus rows: row i = (bearing of center feature pairs[f][i][0], bearing of option feature pairs[f][i][1]).
+struct OptionFrames { uint32_t f[CVB_ARRSAC_BATCH_MAX]; };
+__global__ void __launch_bounds__(256) k_gather_option_bearings(const double *__restrict__ bear, uint32_t cap, uint32_t center, OptionFrames opt,
+                                                                const uint32_t *__restrict__ pairs, const uint32_t *__restrict__ npairs,
+                                                                double *__restrict__ a, double *__restrict__ b) {
+    const uint32_t f = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= min(npairs[f], cap)) return;
+    const uint32_t *p = pairs + ((size_t)f * cap + i) * 2;
+    const double *ba = bear + ((size_t)center * cap + p[0]) * 3, *bb = bear + ((size_t)opt.f[f] * cap + p[1]) * 3;
+    double *da = a + ((size_t)f * cap + i) * 3, *db = b + ((size_t)f * cap + i) * 3;
+    for (int k = 0; k < 3; k++) { da[k] = ba[k]; db[k] = bb[k]; }
+}
+
+int two_view_options_dev(cvb_ctx *ctx, const uint8_t *desc_dev, const uint32_t *n_dev, const double *bearings_dev, uint32_t frames, uint32_t cap,
+                         uint32_t center, const uint32_t *options, uint32_t F, uint32_t better_by, const cvb_arrsac_cfg *cfg, const cvb_rng *rngs,
+                         uint32_t *pairs_out_dev, uint32_t *n_pairs_dev, cvb_pose *model_out_dev, uint32_t *inliers_out_dev,
+                         uint32_t *n_inliers_dev, int32_t *found_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (F == 0) return 0;
+    if (F > CVB_ARRSAC_BATCH_MAX) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "%u options: at most %u", F, CVB_ARRSAC_BATCH_MAX);
+    if (!desc_dev || !n_dev || !bearings_dev || !options || !cfg || !rngs || !pairs_out_dev || !n_pairs_dev || !model_out_dev ||
+        !n_inliers_dev || !found_dev)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (cap == 0) return cvb_set_error(ctx, CVB_EINVAL, "zero capacity");
+    if (center >= frames) return cvb_set_error(ctx, CVB_EINVAL, "center frame %u of %u", center, frames);
+    OptionFrames opt;
+    memset(&opt, 0, sizeof(opt));
+    for (uint32_t f = 0; f < F; f++) {
+        if (options[f] >= frames) return cvb_set_error(ctx, CVB_EINVAL, "option %u: frame %u of %u", f, options[f], frames);
+        opt.f[f] = options[f];
+    }
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    for (uint32_t f = 0; f < F; f++)
+        if ((rc = cvb_match_symmetric_pairs_dev(ctx, desc_dev + (size_t)center * cap * 64, n_dev + center, cap, desc_dev + (size_t)opt.f[f] * cap * 64,
+                                                n_dev + opt.f[f], cap, better_by, pairs_out_dev + (size_t)f * cap * 2, cap, n_pairs_dev + f)))
+            return rc;
+    ArsWorkspace *w = arsws(ctx);
+    if ((rc = w->bdata_a.ensure(ctx, sizeof(double) * 3 * (size_t)F * cap))) return rc;
+    if ((rc = w->bdata_b.ensure(ctx, sizeof(double) * 3 * (size_t)F * cap))) return rc;
+    {
+        CVB_PROF(ctx, "k_gather_option_bearings", 0);
+        k_gather_option_bearings<<<dim3(cdiv(cap, 256), F), 256, 0, ctx->stream>>>(bearings_dev, cap, center, opt, pairs_out_dev, n_pairs_dev,
+                                                                                  (double *)w->bdata_a.p, (double *)w->bdata_b.p);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return arrsac_run_dev_batch(ctx, cfg, 0, (const double *)w->bdata_a.p, (const double *)w->bdata_b.p, n_pairs_dev, cap, cap, F, rngs,
+                                model_out_dev, inliers_out_dev, cap, n_inliers_dev, found_dev, 5, true);
+}
 
 extern "C" {
 
@@ -2607,13 +2803,7 @@ int cvb_arrsac_commit_rng(cvb_ctx *ctx, cvb_rng *rng, uint32_t *stats_out) {
     ArrsacCtl h;
     int rc = arrsac_commit_rng(ctx, rng, &h);
     if (rc) return rc;
-    if (stats_out) {   // 16 words (13..15 reserved): n, valid initial models, SPRT passes, SPRT commit rounds, block iterations, draws, inliers, found, 32-datum units
-                       // scored in stage 1 / stage 2, predicates resolved exactly from the queues, mask words computed by the SPRT itself, SPRT repairs
-        stats_out[0] = h.n; stats_out[1] = h.Mv; stats_out[2] = h.npass; stats_out[3] = h.stat_chunks; stats_out[4] = h.iters;
-        stats_out[5] = (uint32_t)h.rng_pos; stats_out[6] = h.n_inliers; stats_out[7] = h.found;
-        stats_out[8] = h.stat_units0; stats_out[9] = h.stat_units2; stats_out[10] = h.q_count + h.q_count2; stats_out[11] = h.stat_lazy;
-        stats_out[12] = h.stat_repairs; stats_out[13] = h.stat_pad /* data walked by the box walks */; stats_out[14] = h.stat_walk_us; stats_out[15] = h.stat_commit_us;
-    }
+    if (stats_out) arrsac_stats_words(h, stats_out);
     return 0;
 }
 

@@ -7,6 +7,8 @@
   LinearEigenTriangulator and cv-geom's other triangulators: cv_b200/triangulation.py
   Arrsac.model / model_inliers                  <- arrsac::Arrsac as sample_consensus::Consensus
       (call sites akaze/tests/estimate_pose.rs:63-67, lambda-twist/tests/consensus.rs:20,59-61)
+  Arrsac.model_inliers_batch                    <- many independent model_inliers calls, one generator each, in one set of launches
+      (include/cvb200_batch.h; e.g. the candidate frames of cv-sfm's init_reconstruction, cv-sfm/src/lib.rs:966-985)
   Xoshiro256PlusPlus / Pcg64                     <- rand_xoshiro / rand_pcg generators handed to Arrsac::new
 """
 import ctypes as C
@@ -245,6 +247,63 @@ class Arrsac:
             return None
         return np.array(model.r).reshape(3, 3), np.array(model.t), inl[:cnt.value].copy()
 
+    def model_inliers_batch(self, estimator, problems, rngs):
+        """model_inliers of every problem in one batched device run: problems is a list of (a, b) as model_inliers takes them, rngs
+        one generator per problem (each advanced as model_inliers would advance it; self.rng is not used).  Returns a list with one
+        (R, t, inlier indices) or None per problem; problem i equals model_inliers(estimator, *problems[i]) with rngs[i].
+
+        The reference runs such problems one after the other on ONE shared generator; a batch cannot know where each would start,
+        so parity with that shared-generator sequence is unpinned (include/cvb200_batch.h)."""
+        from ._lib import ARRSAC_BATCH_MAX, load_batch_library
+        B = len(problems)
+        if len(rngs) != B:
+            raise ValueError(f"one generator per problem ({len(rngs)} != {B})")
+        if B > ARRSAC_BATCH_MAX:
+            raise ValueError(f"at most {ARRSAC_BATCH_MAX} problems per batch")
+        if B == 0:
+            return []
+        kind, row0, a, b, offsets = pack_arrsac_batch(estimator, problems)
+        BL = load_batch_library()
+        states = (Rng * B)(*[r.state for r in rngs])
+        models = (Pose * B)()
+        inl = np.zeros(max(int(offsets[-1]), 1), np.uint32)
+        cnt = np.zeros(B, np.uint32)
+        found = np.zeros(B, np.int32)
+        self.ctx.check(BL.cvb_arrsac_batch(self.ctx.handle, C.addressof(self.cfg), kind, row0, a.ctypes.data, b.ctypes.data,
+                                           offsets.ctypes.data, B, C.addressof(states), C.addressof(models), inl.ctypes.data,
+                                           cnt.ctypes.data, found.ctypes.data))
+        out = []
+        for i in range(B):
+            C.memmove(C.addressof(rngs[i].state), C.addressof(states[i]), C.sizeof(Rng))
+            if not found[i]:
+                out.append(None)
+                continue
+            o = int(offsets[i])
+            out.append((np.array(models[i].r).reshape(3, 3), np.array(models[i].t), inl[o:o + cnt[i]].copy()))
+        return out
+
     def model(self, estimator, a, b):
         r = self.model_inliers(estimator, a, b)
         return None if r is None else (r[0], r[1])
+
+
+def pack_arrsac_batch(estimator, problems):
+    """(kind, eigenvector_row0, a, b, offsets) of cvb_arrsac_batch: the problems' rows packed one after the other, offsets in CSR form."""
+    if isinstance(estimator, EightPoint):
+        kind, row0, bc = 0, 5, 3
+    elif isinstance(estimator, LambdaTwist):
+        kind, row0, bc = 1, 5, 4
+    elif isinstance(estimator, NisterStewenius):
+        kind, row0, bc = 2, estimator.row0, 3
+    else:
+        raise TypeError("estimator must be EightPoint, LambdaTwist or NisterStewenius")
+    As, Bs = [], []
+    for pa, pb in problems:
+        pa, pb = _f64(pa, 3), _f64(pb, bc)
+        _same_len(pa, pb)
+        As.append(pa); Bs.append(pb)
+    offsets = np.zeros(len(problems) + 1, np.uint32)
+    offsets[1:] = np.cumsum([len(x) for x in As])
+    a = np.ascontiguousarray(np.concatenate(As) if As else np.zeros((0, 3)), np.float64)
+    b = np.ascontiguousarray(np.concatenate(Bs) if Bs else np.zeros((0, bc)), np.float64)
+    return kind, row0, a, b, offsets

@@ -1,12 +1,13 @@
 """cv-sfm's two-view initialisation of one frame pair as ONE call (cv-sfm/src/lib.rs:1375-1412, extraction at :2200-2204):
 AKAZE extract of both frames -> symmetric_matching -> FeatureMatch bearings -> Arrsac + EightPoint, everything on the device,
-one synchronisation at the end (include/cvb200.h: cvb_two_view_frames)."""
+one synchronisation at the end (include/cvb200.h: cvb_two_view_frames).  init_two_view_options: the same initialisation of one frame
+against many candidate frames, with one batched consensus run (include/cvb200_batch.h: cvb_two_view_options_dev)."""
 import ctypes as C
 
 import numpy as np
 
 from ._lib import KP_DTYPE, default_context
-from .geom import Arrsac, Pose, _lib as _geom_lib
+from .geom import Arrsac, Pose, Rng, _lib as _geom_lib
 from .image import is_dynamic
 from .image import lib as _image_lib
 from .image import stack as _stack_frames
@@ -108,3 +109,70 @@ def two_view_frames(akaze, frames, camera, arrsac, better_by=24, cap=8192, buffe
     pose = (np.array(b.model.r).reshape(3, 3), np.array(b.model.t)) if b.found.value else None
     return dict(keypoints=kps, descriptors=descs, matches=b.pairs[:b.n_pairs.value].astype(np.int64), pose=pose,
                 inliers=b.inliers[:b.n_inliers.value].copy() if b.found.value else np.zeros(0, np.uint32))
+
+
+# cv-sfm's default two_view_minimum_robust_matches (cv-sfm/src/settings.rs:393-395)
+TWO_VIEW_MINIMUM_ROBUST_MATCHES = 1 << 8
+
+
+def two_view_option_result(pairs, n_pairs, model_r, model_t, inliers, n_inliers, found, minimum_robust_matches):
+    """One option of init_two_view_options from its device outputs (host copies): None when consensus found nothing or kept fewer
+    than minimum_robust_matches inlier matches (cv-sfm/src/lib.rs:1417-1424), else (R, t, matches), matches = the inlier matches as
+    [center feature, option feature] rows in inlier order (lib.rs:1414)."""
+    if not found or n_inliers < minimum_robust_matches:
+        return None
+    pairs = np.asarray(pairs, np.int64).reshape(-1, 2)[:n_pairs]
+    inl = np.asarray(inliers, np.int64)[:n_inliers]
+    return np.asarray(model_r, np.float64).reshape(3, 3).copy(), np.asarray(model_t, np.float64).copy(), pairs[inl]
+
+
+def init_two_view_options(features, center, options, arrsac, rngs, better_by=24,
+                          minimum_robust_matches=TWO_VIEW_MINIMUM_ROBUST_MATCHES):
+    """cv-sfm's init_two_view(center, option) for every option frame (VSlam::init_reconstruction, cv-sfm/src/lib.rs:966-985 and
+    1365-1432) in one call: F symmetric matches, one gather of the matched bearings, one batched ARRSAC + EightPoint.
+
+    features: device tensors of the frames, as cvb_frame_features_batch_dev leaves them -- "descriptors" [frames, cap, 64] uint8,
+    "counts" [frames] int32 / uint32, "bearings" [frames, cap, 3] float64 (torch CUDA tensors on the context's device).  center, options:
+    frame indices.  arrsac: cv_b200.Arrsac (its configuration; its own generator is not used); rngs: one generator per option, each
+    advanced as model_inliers would advance it.  Returns one result per option: None, or (R, t, matches) with matches the inlier
+    [center feature, option feature] pairs.  Option f equals cvb_two_view_pair_k1_dev on the same frames with rngs[f].  The reference
+    runs the options on one shared generator and shuffles the matches first; parity with that is unpinned."""
+    from ._lib import ARRSAC_BATCH_MAX, load_batch_library
+    import torch
+    desc, cnt, bear = features["descriptors"], features["counts"], features["bearings"]
+    if desc.dtype != torch.uint8 or desc.dim() != 3 or desc.shape[2] != 64 or not desc.is_cuda or not desc.is_contiguous():
+        raise ValueError("descriptors must be a contiguous CUDA uint8 tensor [frames, cap, 64]")
+    frames, cap = desc.shape[0], desc.shape[1]
+    if bear.dtype != torch.float64 or tuple(bear.shape) != (frames, cap, 3) or not bear.is_cuda or not bear.is_contiguous():
+        raise ValueError("bearings must be a contiguous CUDA float64 tensor [frames, cap, 3]")
+    if cnt.dtype not in (torch.int32, torch.uint32) or tuple(cnt.shape) != (frames,) or not cnt.is_cuda:
+        raise ValueError("counts must be a CUDA int32 tensor [frames]")
+    opts = np.ascontiguousarray(options, np.uint32)
+    F = len(opts)
+    if len(rngs) != F:
+        raise ValueError(f"one generator per option ({len(rngs)} != {F})")
+    if F > ARRSAC_BATCH_MAX:
+        raise ValueError(f"at most {ARRSAC_BATCH_MAX} options per call")
+    if F == 0:
+        return []
+    ctx = arrsac.ctx
+    BL = load_batch_library()
+    dev = desc.device
+    pairs = torch.zeros((F, cap, 2), dtype=torch.int32, device=dev)
+    n_pairs = torch.zeros(F, dtype=torch.int32, device=dev)
+    model = torch.zeros((F, 12), dtype=torch.float64, device=dev)
+    inl = torch.zeros((F, cap), dtype=torch.int32, device=dev)
+    n_inl = torch.zeros(F, dtype=torch.int32, device=dev)
+    found = torch.zeros(F, dtype=torch.int32, device=dev)
+    states = (Rng * F)(*[r.state for r in rngs])
+    torch.cuda.synchronize(dev)
+    ctx.check(BL.cvb_two_view_options_dev(ctx.handle, desc.data_ptr(), cnt.data_ptr(), bear.data_ptr(), frames, cap, int(center),
+                                          opts.ctypes.data, F, better_by, C.addressof(arrsac.cfg), C.addressof(states), pairs.data_ptr(),
+                                          n_pairs.data_ptr(), model.data_ptr(), inl.data_ptr(), n_inl.data_ptr(), found.data_ptr()))
+    ctx.check(BL.cvb_arrsac_commit_rng_batch(ctx.handle, C.addressof(states), F, None))
+    for f in range(F):
+        C.memmove(C.addressof(rngs[f].state), C.addressof(states[f]), C.sizeof(Rng))
+    pairs, n_pairs, model = pairs.cpu().numpy(), n_pairs.cpu().numpy(), model.cpu().numpy()
+    inl, n_inl, found = inl.cpu().numpy(), n_inl.cpu().numpy(), found.cpu().numpy()
+    return [two_view_option_result(pairs[f], int(n_pairs[f]), model[f, :9], model[f, 9:], inl[f], int(n_inl[f]), int(found[f]),
+                                   minimum_robust_matches) for f in range(F)]
