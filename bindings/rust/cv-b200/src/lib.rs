@@ -204,3 +204,6 @@ pub mod stages;
 
 // ---- INTEGRATION.md section 2k (include/cvb200_batch.h) ----
 pub mod batch;
+
+// ---- INTEGRATION.md section 2l (include/cvb200_init.h) ----
+pub mod init;

@@ -18,6 +18,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   frame_features        <- cv-sfm VSlam::kps_descriptors        (cv-sfm/src/lib.rs:2195-2235)
   init_two_view_options <- cv-sfm init_two_view against every candidate frame (cv-sfm/src/lib.rs:966-985, 1365-1432), one batched
                            consensus run (Arrsac.model_inliers_batch: many independent model_inliers calls)
+  init_reconstruction, InitSettings <- cv-sfm VSlam::init_reconstruction (cv-sfm/src/lib.rs:966-1303): the two-view options and the
+                           three-view choice over every pair of them, chained on the device
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -42,7 +44,8 @@ from .optimize import (observation_losses, single_view_simple_optimize_l1, singl
                        three_view_simple_optimize_l2, tri_landmarks_robust)
 from .sfm_match import landmark_matches  # noqa: F401
 from . import checkpoint  # noqa: F401  (bincode record images of the VSlamData checkpoint)
-from .pair import Intrinsics, IntrinsicsK1, TwoViewBuffers, init_two_view_options, two_view_frames  # noqa: F401
+from .pair import (InitSettings, Intrinsics, IntrinsicsK1, TwoViewBuffers, init_reconstruction, init_two_view_options,  # noqa: F401
+                   two_view_frames)
 from .features import frame_features  # noqa: F401
 
 __version__ = "0.1.0"

@@ -1,7 +1,8 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
 (include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
-cv_b200/libcvb200_stages.so (include/cvb200_stages.h) and cv_b200/libcvb200_batch.so (include/cvb200_batch.h)."""
+cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h) and cv_b200/libcvb200_init.so
+(include/cvb200_init.h)."""
 import ctypes as C
 import os
 
@@ -114,6 +115,10 @@ BATCH_ABI_SYMBOLS = [
 ]
 # CVB_ARRSAC_BATCH_MAX of include/cvb200_batch.h
 ARRSAC_BATCH_MAX = 64
+
+# every symbol include/cvb200_init.h declares (cv-sfm's three-view initialisation), exported by libcvb200_init.so; checked by
+# tests/test_abi_init.py
+INIT_ABI_SYMBOLS = ["cvb_init_cfg_default", "cvb_init_reconstruction_dev"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -319,6 +324,30 @@ def load_batch_library():
         L.cvb_two_view_options_dev.argtypes = [vp, vp, vp, vp, u32, u32, u32, vp, u32, u32, vp, vp, vp, vp, vp, vp, vp, vp]
         _BATCH_LIB = L
     return _BATCH_LIB
+
+
+_INIT_LIB = None
+
+
+def init_lib_path():
+    return os.path.join(_HERE, "libcvb200_init.so")
+
+
+def load_init_library():
+    """Loads libcvb200_init.so, the module of include/cvb200_init.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _INIT_LIB
+    if _INIT_LIB is None:
+        load_library()
+        p = init_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_init_cfg_default.argtypes = [vp]
+        L.cvb_init_cfg_default.restype = None
+        L.cvb_init_reconstruction_dev.argtypes = [vp, vp, vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+        _INIT_LIB = L
+    return _INIT_LIB
 
 
 class Context:

@@ -6,6 +6,7 @@
 // consumes bit-packed inlier masks.  Reference lines are cited per function (paths relative to the reference checkout).
 // The linear algebra that lives in nalgebra upstream (symmetric eigen, SVD, from_matrix_eps) is implemented
 // here as cyclic Jacobi / closed forms; f64 results are held to 1e-6 relative (BASELINE north_star) in the parity tests.
+#include <float.h>
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -17,6 +18,7 @@
 #include "../../include/cvb200_opt.h"
 #include "../../include/cvb200_pinhole.h"
 #include "../../include/cvb200_batch.h"
+#include "../../include/cvb200_init.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1478,19 +1480,17 @@ __global__ void __launch_bounds__(128) k_observation_losses(cvb_triangulator T, 
     const bool ok = triangulate_observations(T, P, B, n, W ? W + 6 * (size_t)o0 : nullptr, p);
     for (uint32_t i = 0; i < n; i++) loss[o0 + i] = ok ? transformed_cosine_distance(P[i], p, B + 3 * (size_t)i) : 2.0;
 }
-// cv-sfm/src/lib.rs:1320-1360 is_tri_landmark_robust with the triangulator T; one thread per (centre, first, second) observation
-// triple of one pose pair
-__global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T, cvb_pose first, cvb_pose second, const double *__restrict__ obs,
-                                                             uint32_t n, double max_cos, double inc_min_cos, uint8_t *__restrict__ out) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const double *c = obs + 9 * (size_t)i, *f = c + 3, *s = c + 6;
+// cv-sfm/src/lib.rs:1320-1360 is_tri_landmark_robust with the triangulator T (poses CameraToCamera centre -> first / second);
+// B: the centre, first and second bearings, contiguous
+__device__ bool tri_landmark_robust(const cvb_triangulator &T, const cvb_pose &first, const cvb_pose &second, const double *B, double max_cos,
+                                    double inc_min_cos) {
+    const double *c = B, *f = B + 3, *s = B + 6;
     cvb_pose P[3];
     for (int k = 0; k < 9; k++) P[0].r[k] = (k % 4 == 0) ? 1.0 : 0.0;
     P[0].t[0] = P[0].t[1] = P[0].t[2] = 0.0;
     P[1] = first; P[2] = second;
     double p[4], W[18];
-    if (!triangulate_observations(T, P, c, 3, W, p)) { out[i] = 0; return; }
+    if (!triangulate_observations(T, P, c, 3, W, p)) return false;
     from_homogeneous(p);   // CameraPoint::from_homogeneous(p.0)
     double fc[3], sc[3];
     for (int k = 0; k < 3; k++) {
@@ -1500,8 +1500,17 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
     const bool cosine_ok = 1.0 - dot3(p, c) < max_cos && transformed_cosine_distance(first, p, f) < max_cos
         && transformed_cosine_distance(second, p, s) < max_cos;
     const bool incidence_ok = 1.0 - dot3(c, fc) > inc_min_cos || 1.0 - dot3(c, sc) > inc_min_cos || 1.0 - dot3(fc, sc) > inc_min_cos;
-    out[i] = cosine_ok && incidence_ok;
+    return cosine_ok && incidence_ok;
 }
+// one thread per (centre, first, second) observation triple of one pose pair
+__global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T, cvb_pose first, cvb_pose second, const double *__restrict__ obs,
+                                                             uint32_t n, double max_cos, double inc_min_cos, uint8_t *__restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    out[i] = tri_landmark_robust(T, first, second, obs + 9 * (size_t)i, max_cos, inc_min_cos);
+}
+
+#include "init_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1659,11 +1668,12 @@ struct ArsWorkspace {
 };
 struct GeomWorkspace {
     DevBuf a, b, samples, poses, nposes, out, masks, offsets, ok;
+    DevBuf init;                    // the three-view initialisation's per-call workspace (init_reconstruction_dev)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
-    DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok};
+    DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -2557,6 +2567,200 @@ int two_view_options_dev(cvb_ctx *ctx, const uint8_t *desc_dev, const uint32_t *
     }
     return arrsac_run_dev_batch(ctx, cfg, 0, (const double *)w->bdata_a.p, (const double *)w->bdata_b.p, n_pairs_dev, cap, cap, F, rngs,
                                 model_out_dev, inliers_out_dev, cap, n_inliers_dev, found_dev, 5, true);
+}
+
+// ---- cv-sfm's three-view initialisation (C names in init_abi.cu, include/cvb200_init.h; kernels in init_dev.cuh) -------------
+void init_cfg_default(cvb_init_cfg *c) {
+    if (!c) return;
+    memset(c, 0, sizeof(*c));
+    c->robust_observation_incidence_minimum_cosine_distance = 1e-3;
+    c->robust_view_bearing_pair_minimum_cosine_distance = 1e-2;
+    c->maximum_cosine_distance = 1e-5;
+    c->maximum_sine_distance = 1e-1;
+    c->two_view_minimum_robust_matches = 1u << 8;
+    c->three_view_minimum_relative_scales = 1u << 4;
+    c->three_view_optimization_landmarks = 1u << 10;
+    c->robust_view_num_robust_bearing_pair = 3;
+    c->three_view_filter_loop_iterations = 1u << 3;
+    c->three_view_patience = 1u << 16;
+    c->three_view_minimum_robust_matches = 32;
+}
+
+static size_t init_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+int init_reconstruction_dev(cvb_ctx *ctx, const cvb_init_cfg *cfg, const cvb_triangulator *tri, const double *bearings_dev, uint32_t frames,
+                            uint32_t cap, uint32_t center, const uint32_t *options, uint32_t F, const uint32_t *pairs_dev,
+                            const uint32_t *n_pairs_dev, const cvb_pose *model_dev, const uint32_t *inliers_dev, const uint32_t *n_inliers_dev,
+                            const int32_t *found_dev, cvb_init_result *result_dev, uint32_t *combined_dev, uint32_t *first_matches_dev,
+                            uint32_t *second_matches_dev, cvb_init_pair_stats *stats_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !bearings_dev || !pairs_dev || !n_pairs_dev || !model_dev || !inliers_dev || !n_inliers_dev || !found_dev ||
+        !result_dev || !combined_dev || !first_matches_dev || !second_matches_dev || (F && !options))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (F > CVB_ARRSAC_BATCH_MAX) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "%u options: at most %u", F, CVB_ARRSAC_BATCH_MAX);
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: init_reconstruction takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (cap == 0) return cvb_set_error(ctx, CVB_EINVAL, "zero capacity");
+    if (center >= frames) return cvb_set_error(ctx, CVB_EINVAL, "center frame %u of %u", center, frames);
+    InitFrames fr;
+    memset(&fr, 0, sizeof(fr));
+    fr.center = center;
+    for (uint32_t f = 0; f < F; f++) {
+        if (options[f] >= frames) return cvb_set_error(ctx, CVB_EINVAL, "option %u: frame %u of %u", f, options[f], frames);
+        fr.f[f] = options[f];
+    }
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int W = 0;
+    CVB_CUDA(ctx, cudaDeviceGetAttribute(&W, cudaDevAttrMultiProcessorCount, ctx->device));
+    const uint32_t Fm = std::max<uint32_t>(F, 1), L = std::max<uint32_t>(std::min(cfg->three_view_optimization_landmarks, cap), 1);
+    uint32_t n2 = 1;
+    while (n2 < cap) n2 <<= 1;
+    // workspace: control | W slots | maps | W x (common triples, 3 flag planes, ratios, sort buffer, optimisation rows) | offsets | poses
+    size_t off = 0;
+    const size_t o_ctl = off; off += init_align(sizeof(InitCtl));
+    const size_t o_slots = off; off += init_align(sizeof(InitSlot) * W);
+    const size_t o_map = off; off += init_align(sizeof(uint32_t) * (size_t)Fm * cap);
+    const size_t o_common = off; off += init_align(sizeof(uint32_t) * 3 * (size_t)W * cap);
+    const size_t o_flags = off; off += init_align((size_t)W * cap);
+    const size_t o_ff = off; off += init_align((size_t)W * cap);
+    const size_t o_fs = off; off += init_align((size_t)W * cap);
+    const size_t o_ratio = off; off += init_align(sizeof(double) * (size_t)W * cap);
+    const size_t o_sort = off; off += init_align(sizeof(double) * (size_t)W * n2);
+    const size_t o_obs = off; off += init_align(sizeof(double) * 9 * (size_t)W * L);
+    const size_t o_offs = off; off += init_align(sizeof(uint32_t) * (W + 1));
+    const size_t o_poses = off; off += init_align(sizeof(cvb_pose) * 2 * (size_t)W);
+    const size_t o_popt = off; off += init_align(sizeof(cvb_pose) * 2 * (size_t)W);
+    const size_t o_upd = off; off += init_align(sizeof(uint32_t) * W);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->init.ensure(ctx, off))) return rc;
+    unsigned char *base = (unsigned char *)g->init.p;
+    InitCtl *ctl = (InitCtl *)(base + o_ctl);
+    InitSlot *slots = (InitSlot *)(base + o_slots);
+    uint32_t *map = (uint32_t *)(base + o_map), *common = (uint32_t *)(base + o_common), *offs = (uint32_t *)(base + o_offs);
+    uint8_t *flags = base + o_flags, *ffirst = base + o_ff, *fsecond = base + o_fs;
+    double *ratio = (double *)(base + o_ratio), *sortbuf = (double *)(base + o_sort), *obs = (double *)(base + o_obs);
+    cvb_pose *poses = (cvb_pose *)(base + o_poses), *popt = (cvb_pose *)(base + o_popt);
+    uint32_t *upd = (uint32_t *)(base + o_upd);
+    InitParams prm;
+    prm.inc = cfg->robust_observation_incidence_minimum_cosine_distance;
+    prm.bp_min_cos = cfg->robust_view_bearing_pair_minimum_cosine_distance;
+    prm.max_cos = cfg->maximum_cosine_distance;
+    prm.max_sine = cfg->maximum_sine_distance;
+    prm.min_scales = cfg->three_view_minimum_relative_scales;
+    prm.limit = cfg->three_view_optimization_landmarks;
+    prm.bp_min = cfg->robust_view_num_robust_bearing_pair;
+    prm.min_robust = cfg->three_view_minimum_robust_matches;
+    const cvb_triangulator T = *tri;
+    const uint32_t npairs_max = F * (F - (F > 0)) / 2;
+    cudaStream_t st = ctx->stream;
+    {
+        CVB_PROF(ctx, "k_init_setup", 0);
+        if (stats_dev && npairs_max) CVB_CUDA(ctx, cudaMemsetAsync(stats_dev, 0, sizeof(cvb_init_pair_stats) * npairs_max, st));
+        CVB_CUDA(ctx, cudaMemsetAsync(map, 0xff, sizeof(uint32_t) * (size_t)Fm * cap, st));
+        k_init_setup<<<1, 32, 0, st>>>(n_inliers_dev, found_dev, F, cfg->two_view_minimum_robust_matches, ctl);
+        CVB_LAUNCH_CHECK(ctx);
+        if (F) {
+            k_init_maps<<<dim3(cdiv(cap, 256), F), 256, 0, st>>>(pairs_dev, inliers_dev, n_inliers_dev, found_dev, cap, map);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+    }
+    const dim3 gtri(cdiv(cap, 128), W), gslot(cdiv(W, 128));
+    uint32_t *h = (uint32_t *)cvb_pinned(ctx, 4 * sizeof(uint32_t));   // K, P, decided, slot of the control block
+    if (!h) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    // the pairs that exist are known on the device only: wave 0 runs whenever F >= 2, and its readback bounds the rest
+    uint32_t npairs = npairs_max;
+    for (uint32_t wave = 0; wave * (uint32_t)W < npairs; wave++) {
+        {
+            CVB_PROF(ctx, "k_init_begin", 0);
+            k_init_begin<<<gslot, 128, 0, st>>>(ctl, wave * W, W, model_dev, slots, poses);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        {
+            CVB_PROF(ctx, "k_init_common", 0);
+            k_init_common<<<W, 256, 0, st>>>(pairs_dev, inliers_dev, n_inliers_dev, map, cap, slots, common);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        {
+            CVB_PROF(ctx, "k_init_flags_scale", 0);
+            k_init_flags<0><<<gtri, 128, 0, st>>>(T, bearings_dev, cap, fr, common, poses, prm, 1.0, slots, flags, ratio);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        {
+            CVB_PROF(ctx, "k_init_median", 0);
+            k_init_median<<<W, 256, 0, st>>>(cap, n2, prm, flags, ratio, slots, sortbuf, poses);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        auto opti_set = [&](bool reflag, double max_cos, uint32_t mode) -> int {
+            if (reflag) {
+                CVB_PROF(ctx, "k_init_flags_opti", 0);
+                k_init_flags<1><<<gtri, 128, 0, st>>>(T, bearings_dev, cap, fr, common, poses, prm, max_cos, slots, flags, ratio);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            {
+                CVB_PROF(ctx, "k_init_sizes", 0);
+                k_init_sizes<<<1, 32, 0, st>>>(W, mode, prm, slots, offs);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            {
+                CVB_PROF(ctx, "k_init_gather", 0);
+                k_init_gather<<<W, 256, 0, st>>>(bearings_dev, cap, fr, common, flags, slots, offs, obs);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            return 0;
+        };
+        auto optimise = [&]() -> int {
+            {
+                CVB_PROF(ctx, "k_three_view_opt", 0);
+                k_three_view_opt<<<W, OPT_NT, 0, st>>>(poses, obs, offs, 0, 0.001, cfg->three_view_patience, popt, upd);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            {
+                CVB_PROF(ctx, "k_init_post_opt", 0);
+                k_init_post_opt<<<gslot, 128, 0, st>>>(W, popt, upd, slots, poses);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            return 0;
+        };
+        // lib.rs:1064-1106: the first set (under the scaled poses) and its robust bearing pairs
+        if ((rc = opti_set(true, 1.0, INIT_SZ_RECOUNT | INIT_SZ_FIRST))) return rc;
+        {
+            CVB_PROF(ctx, "k_init_bearing_pairs", 0);
+            k_init_bearing_pairs<<<dim3(cdiv(L, 128), W), 128, 0, st>>>(obs, offs, prm.bp_min_cos, slots);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        // lib.rs:1112-1187: the filter loop and the final optimisation; the first check reuses the first set
+        if ((rc = opti_set(false, 0.0, INIT_SZ_BEARING | INIT_SZ_CHECK))) return rc;
+        for (uint32_t it = 0; it < cfg->three_view_filter_loop_iterations; it++) {
+            if ((rc = optimise())) return rc;
+            if ((rc = opti_set(true, prm.max_cos, INIT_SZ_RECOUNT | INIT_SZ_CHECK))) return rc;
+        }
+        if ((rc = optimise())) return rc;
+        {
+            CVB_PROF(ctx, "k_init_final", 0);
+            k_init_flags<2><<<gtri, 128, 0, st>>>(T, bearings_dev, cap, fr, common, poses, prm, prm.max_cos, slots, flags, ratio);
+            CVB_LAUNCH_CHECK(ctx);
+            k_init_bi_flags<<<dim3(cdiv(cap, 128), W, 2), 128, 0, st>>>(bearings_dev, cap, fr, pairs_dev, inliers_dev, n_inliers_dev, map, poses,
+                                                                        prm, slots, ffirst, fsecond);
+            CVB_LAUNCH_CHECK(ctx);
+            k_init_accept<<<gslot, 128, 0, st>>>(W, prm, slots);
+            CVB_LAUNCH_CHECK(ctx);
+            k_init_decide<<<1, 32, 0, st>>>(W, slots, ctl, stats_dev);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        CVB_CUDA(ctx, cudaMemcpyAsync(h, ctl, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        if ((int32_t)h[2] >= 0) break;
+        npairs = h[1];
+    }
+    {
+        CVB_PROF(ctx, "k_init_finish", 0);
+        k_init_finish<<<1, 256, 0, st>>>(ctl, slots, cap, pairs_dev, inliers_dev, n_inliers_dev, common, flags, ffirst, fsecond, poses, result_dev,
+                                         combined_dev, first_matches_dev, second_matches_dev);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return 0;
 }
 
 extern "C" {

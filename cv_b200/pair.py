@@ -1,7 +1,8 @@
 """cv-sfm's two-view initialisation of one frame pair as ONE call (cv-sfm/src/lib.rs:1375-1412, extraction at :2200-2204):
 AKAZE extract of both frames -> symmetric_matching -> FeatureMatch bearings -> Arrsac + EightPoint, everything on the device,
 one synchronisation at the end (include/cvb200.h: cvb_two_view_frames).  init_two_view_options: the same initialisation of one frame
-against many candidate frames, with one batched consensus run (include/cvb200_batch.h: cvb_two_view_options_dev)."""
+against many candidate frames, with one batched consensus run (include/cvb200_batch.h: cvb_two_view_options_dev).  init_reconstruction:
+cv-sfm's three-view initialisation over those options, chained on the device (include/cvb200_init.h: cvb_init_reconstruction_dev)."""
 import ctypes as C
 
 import numpy as np
@@ -126,17 +127,9 @@ def two_view_option_result(pairs, n_pairs, model_r, model_t, inliers, n_inliers,
     return np.asarray(model_r, np.float64).reshape(3, 3).copy(), np.asarray(model_t, np.float64).copy(), pairs[inl]
 
 
-def init_two_view_options(features, center, options, arrsac, rngs, better_by=24,
-                          minimum_robust_matches=TWO_VIEW_MINIMUM_ROBUST_MATCHES):
-    """cv-sfm's init_two_view(center, option) for every option frame (VSlam::init_reconstruction, cv-sfm/src/lib.rs:966-985 and
-    1365-1432) in one call: F symmetric matches, one gather of the matched bearings, one batched ARRSAC + EightPoint.
-
-    features: device tensors of the frames, as cvb_frame_features_batch_dev leaves them -- "descriptors" [frames, cap, 64] uint8,
-    "counts" [frames] int32 / uint32, "bearings" [frames, cap, 3] float64 (torch CUDA tensors on the context's device).  center, options:
-    frame indices.  arrsac: cv_b200.Arrsac (its configuration; its own generator is not used); rngs: one generator per option, each
-    advanced as model_inliers would advance it.  Returns one result per option: None, or (R, t, matches) with matches the inlier
-    [center feature, option feature] pairs.  Option f equals cvb_two_view_pair_k1_dev on the same frames with rngs[f].  The reference
-    runs the options on one shared generator and shuffles the matches first; parity with that is unpinned."""
+def _two_view_options_dev(features, center, options, arrsac, rngs, better_by):
+    """The checks and the device call shared by init_two_view_options and init_reconstruction: runs cvb_two_view_options_dev, commits
+    the generators, and returns (frames, cap, opts, device outputs dict) -- the outputs stay on the device.  None when F = 0."""
     from ._lib import ARRSAC_BATCH_MAX, load_batch_library
     import torch
     desc, cnt, bear = features["descriptors"], features["counts"], features["bearings"]
@@ -154,25 +147,134 @@ def init_two_view_options(features, center, options, arrsac, rngs, better_by=24,
     if F > ARRSAC_BATCH_MAX:
         raise ValueError(f"at most {ARRSAC_BATCH_MAX} options per call")
     if F == 0:
-        return []
+        return frames, cap, opts, None
     ctx = arrsac.ctx
     BL = load_batch_library()
     dev = desc.device
-    pairs = torch.zeros((F, cap, 2), dtype=torch.int32, device=dev)
-    n_pairs = torch.zeros(F, dtype=torch.int32, device=dev)
-    model = torch.zeros((F, 12), dtype=torch.float64, device=dev)
-    inl = torch.zeros((F, cap), dtype=torch.int32, device=dev)
-    n_inl = torch.zeros(F, dtype=torch.int32, device=dev)
-    found = torch.zeros(F, dtype=torch.int32, device=dev)
+    out = dict(pairs=torch.zeros((F, cap, 2), dtype=torch.int32, device=dev), n_pairs=torch.zeros(F, dtype=torch.int32, device=dev),
+               model=torch.zeros((F, 12), dtype=torch.float64, device=dev), inliers=torch.zeros((F, cap), dtype=torch.int32, device=dev),
+               n_inliers=torch.zeros(F, dtype=torch.int32, device=dev), found=torch.zeros(F, dtype=torch.int32, device=dev))
     states = (Rng * F)(*[r.state for r in rngs])
     torch.cuda.synchronize(dev)
     ctx.check(BL.cvb_two_view_options_dev(ctx.handle, desc.data_ptr(), cnt.data_ptr(), bear.data_ptr(), frames, cap, int(center),
-                                          opts.ctypes.data, F, better_by, C.addressof(arrsac.cfg), C.addressof(states), pairs.data_ptr(),
-                                          n_pairs.data_ptr(), model.data_ptr(), inl.data_ptr(), n_inl.data_ptr(), found.data_ptr()))
+                                          opts.ctypes.data, F, better_by, C.addressof(arrsac.cfg), C.addressof(states),
+                                          out["pairs"].data_ptr(), out["n_pairs"].data_ptr(), out["model"].data_ptr(),
+                                          out["inliers"].data_ptr(), out["n_inliers"].data_ptr(), out["found"].data_ptr()))
     ctx.check(BL.cvb_arrsac_commit_rng_batch(ctx.handle, C.addressof(states), F, None))
     for f in range(F):
         C.memmove(C.addressof(rngs[f].state), C.addressof(states[f]), C.sizeof(Rng))
-    pairs, n_pairs, model = pairs.cpu().numpy(), n_pairs.cpu().numpy(), model.cpu().numpy()
-    inl, n_inl, found = inl.cpu().numpy(), n_inl.cpu().numpy(), found.cpu().numpy()
+    return frames, cap, opts, out
+
+
+def init_two_view_options(features, center, options, arrsac, rngs, better_by=24,
+                          minimum_robust_matches=TWO_VIEW_MINIMUM_ROBUST_MATCHES):
+    """cv-sfm's init_two_view(center, option) for every option frame (VSlam::init_reconstruction, cv-sfm/src/lib.rs:966-985 and
+    1365-1432) in one call: F symmetric matches, one gather of the matched bearings, one batched ARRSAC + EightPoint.
+
+    features: device tensors of the frames, as cvb_frame_features_batch_dev leaves them -- "descriptors" [frames, cap, 64] uint8,
+    "counts" [frames] int32 / uint32, "bearings" [frames, cap, 3] float64 (torch CUDA tensors on the context's device).  center, options:
+    frame indices.  arrsac: cv_b200.Arrsac (its configuration; its own generator is not used); rngs: one generator per option, each
+    advanced as model_inliers would advance it.  Returns one result per option: None, or (R, t, matches) with matches the inlier
+    [center feature, option feature] pairs.  Option f equals cvb_two_view_pair_k1_dev on the same frames with rngs[f].  The reference
+    runs the options on one shared generator and shuffles the matches first; parity with that is unpinned."""
+    _, _, opts, out = _two_view_options_dev(features, center, options, arrsac, rngs, better_by)
+    if out is None:
+        return []
+    pairs, n_pairs, model = out["pairs"].cpu().numpy(), out["n_pairs"].cpu().numpy(), out["model"].cpu().numpy()
+    inl, n_inl, found = out["inliers"].cpu().numpy(), out["n_inliers"].cpu().numpy(), out["found"].cpu().numpy()
     return [two_view_option_result(pairs[f], int(n_pairs[f]), model[f, :9], model[f, 9:], inl[f], int(n_inl[f]), int(found[f]),
-                                   minimum_robust_matches) for f in range(F)]
+                                   minimum_robust_matches) for f in range(len(opts))]
+
+
+class InitSettings(C.Structure):
+    """cvb_init_cfg: the cv-sfm settings init_reconstruction reads, with their defaults (cv-sfm/src/settings.rs:320-428)."""
+    _fields_ = [("robust_observation_incidence_minimum_cosine_distance", C.c_double),
+                ("robust_view_bearing_pair_minimum_cosine_distance", C.c_double), ("maximum_cosine_distance", C.c_double),
+                ("maximum_sine_distance", C.c_double), ("two_view_minimum_robust_matches", C.c_uint32),
+                ("three_view_minimum_relative_scales", C.c_uint32), ("three_view_optimization_landmarks", C.c_uint32),
+                ("robust_view_num_robust_bearing_pair", C.c_uint32), ("three_view_filter_loop_iterations", C.c_uint32),
+                ("three_view_patience", C.c_uint32), ("three_view_minimum_robust_matches", C.c_uint32), ("reserved", C.c_uint32)]
+
+    def __init__(self, **kw):
+        d = dict(robust_observation_incidence_minimum_cosine_distance=1e-3, robust_view_bearing_pair_minimum_cosine_distance=1e-2,
+                 maximum_cosine_distance=1e-5, maximum_sine_distance=0.1, two_view_minimum_robust_matches=TWO_VIEW_MINIMUM_ROBUST_MATCHES,
+                 three_view_minimum_relative_scales=16, three_view_optimization_landmarks=1024, robust_view_num_robust_bearing_pair=3,
+                 three_view_filter_loop_iterations=8, three_view_patience=1 << 16, three_view_minimum_robust_matches=32)
+        d.update(kw)
+        super().__init__(**d)
+
+
+POSE_DTYPE = np.dtype([("r", "<f8", (9,)), ("t", "<f8", (3,))])
+# cvb_init_result and cvb_init_pair_stats (include/cvb200_init.h)
+INIT_RESULT_DTYPE = np.dtype([("status", "<i4"), ("pair", "<u4"), ("first", "<u4"), ("second", "<u4"), ("n_pairs", "<u4"),
+                              ("n_combined", "<u4"), ("n_first_matches", "<u4"), ("n_second_matches", "<u4"), ("first_pose", POSE_DTYPE),
+                              ("second_pose", POSE_DTYPE)])
+INIT_PAIR_STATS_DTYPE = np.dtype([("outcome", "<i4"), ("first", "<u4"), ("second", "<u4"), ("scales", "<u4"), ("median_scale", "<f8"),
+                                  ("bearing_pairs", "<u8"), ("common", "<u4"), ("opti", "<u4"), ("updates", "<u4"), ("robust", "<u4")])
+
+
+def init_reconstruction_dev(ctx, features_bearings, center, options, two_view, settings=None, triangulator=None, stats=False):
+    """cvb_init_reconstruction_dev on device tensors: features_bearings [frames, cap, 3] float64 (CUDA), two_view: the device outputs of
+    cvb_two_view_options_dev for the same center / options (dict pairs, n_pairs, model, inliers, n_inliers, found).  Returns host copies:
+    dict(result (INIT_RESULT_DTYPE record), combined [n, 3], first_matches [n, 2], second_matches [n, 2], stats (or None))."""
+    from ._lib import load_init_library
+    from .triangulation import LinearEigenTriangulator
+    import torch
+    bear = features_bearings
+    if bear.dtype != torch.float64 or bear.dim() != 3 or bear.shape[2] != 3 or not bear.is_cuda or not bear.is_contiguous():
+        raise ValueError("bearings must be a contiguous CUDA float64 tensor [frames, cap, 3]")
+    frames, cap = bear.shape[0], bear.shape[1]
+    opts = np.ascontiguousarray(options, np.uint32)
+    F = len(opts)
+    settings = settings if settings is not None else InitSettings()
+    tri = triangulator if triangulator is not None else LinearEigenTriangulator()
+    dev = bear.device
+    res = torch.zeros(INIT_RESULT_DTYPE.itemsize, dtype=torch.uint8, device=dev)
+    comb = torch.zeros((cap, 3), dtype=torch.int32, device=dev)
+    fm = torch.zeros((cap, 2), dtype=torch.int32, device=dev)
+    sm = torch.zeros((cap, 2), dtype=torch.int32, device=dev)
+    npairs = F * (F - 1) // 2
+    st = torch.zeros(max(npairs, 1) * INIT_PAIR_STATS_DTYPE.itemsize, dtype=torch.uint8, device=dev) if stats else None
+    if two_view is None:
+        z = torch.zeros(max(F, 1) * cap * 2, dtype=torch.int32, device=dev)
+        two_view = dict(pairs=z, n_pairs=z, model=torch.zeros((1, 12), dtype=torch.float64, device=dev), inliers=z, n_inliers=z, found=z)
+    IL = load_init_library()
+    torch.cuda.synchronize(dev)
+    ctx.check(IL.cvb_init_reconstruction_dev(ctx.handle, C.addressof(settings), C.addressof(tri.cfg), bear.data_ptr(), frames, cap, int(center),
+                                             opts.ctypes.data if F else None, F, two_view["pairs"].data_ptr(), two_view["n_pairs"].data_ptr(),
+                                             two_view["model"].data_ptr(), two_view["inliers"].data_ptr(), two_view["n_inliers"].data_ptr(),
+                                             two_view["found"].data_ptr(), res.data_ptr(), comb.data_ptr(), fm.data_ptr(), sm.data_ptr(),
+                                             st.data_ptr() if st is not None else None))
+    torch.cuda.synchronize(dev)
+    r = np.frombuffer(res.cpu().numpy().tobytes(), INIT_RESULT_DTYPE)[0]
+    return dict(result=r, combined=comb[:int(r["n_combined"])].cpu().numpy().astype(np.int64),
+                first_matches=fm[:int(r["n_first_matches"])].cpu().numpy().astype(np.int64),
+                second_matches=sm[:int(r["n_second_matches"])].cpu().numpy().astype(np.int64),
+                stats=np.frombuffer(st.cpu().numpy().tobytes(), INIT_PAIR_STATS_DTYPE)[:npairs].copy() if st is not None else None)
+
+
+def init_reconstruction(features, center, options, arrsac, rngs, settings=None, triangulator=None, better_by=24):
+    """cv-sfm's VSlam::init_reconstruction (cv-sfm/src/lib.rs:966-1303) of frame `center` against the option frames, on the device:
+    init_two_view against every option (init_two_view_options) and the choice of the three-view initialisation over every pair of the
+    options that pass (include/cvb200_init.h), with no host copy between them.
+
+    features, center, options, arrsac, rngs, better_by: as init_two_view_options.  settings: InitSettings (cv-sfm's defaults);
+    triangulator: a TriangulatorObservations (LinearEigenTriangulator, SineL1Triangulator or MeanMeanTriangulator; default
+    LinearEigen).  Returns None, or dict(first, first_pose, second, second_pose, combined, first_matches, second_matches) with first /
+    second the chosen frames, poses (R, t) CameraToCamera center -> frame, combined [n, 3] (center, first, second feature) and the two
+    [n, 2] (center, option feature) lists.  Unpinned: the reference shuffles the common matches (lib.rs:999) and the matches in front of
+    consensus with one shared generator; here they keep their order, and each option has its own generator."""
+    settings = settings if settings is not None else InitSettings()
+    if triangulator is not None and getattr(triangulator, "method", None) not in (0, 1, 2):
+        raise ValueError("init_reconstruction takes a TriangulatorObservations: LinearEigen, SineL1 or MeanMean")
+    frames, cap, opts, out = _two_view_options_dev(features, center, options, arrsac, rngs, better_by)
+    r = init_reconstruction_dev(arrsac.ctx, features["bearings"], center, opts, out, settings, triangulator)
+    res = r["result"]
+    if res["status"] != 1:
+        return None
+
+    def pose(p):
+        return np.array(p["r"]).reshape(3, 3), np.array(p["t"])
+    return dict(first=int(opts[res["first"]]), first_pose=pose(res["first_pose"]), second=int(opts[res["second"]]),
+                second_pose=pose(res["second_pose"]), combined=r["combined"], first_matches=r["first_matches"],
+                second_matches=r["second_matches"])
