@@ -207,3 +207,6 @@ pub mod batch;
 
 // ---- INTEGRATION.md section 2l (include/cvb200_init.h) ----
 pub mod init;
+
+// ---- INTEGRATION.md section 2m (include/cvb200_constraints.h) ----
+pub mod constraints;

@@ -20,6 +20,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
                            consensus run (Arrsac.model_inliers_batch: many independent model_inliers calls)
   init_reconstruction, InitSettings <- cv-sfm VSlam::init_reconstruction (cv-sfm/src/lib.rs:966-1303): the two-view options and the
                            three-view choice over every pair of them, chained on the device
+  generate_view_constraints, ConstraintSettings <- cv-sfm VSlam::generate_view_constraints / record_view_constraints
+                           (cv-sfm/src/lib.rs:2092-2109, 2438-2516) for many views of one reconstruction snapshot in one call
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -47,5 +49,6 @@ from . import checkpoint  # noqa: F401  (bincode record images of the VSlamData 
 from .pair import (InitSettings, Intrinsics, IntrinsicsK1, TwoViewBuffers, init_reconstruction, init_two_view_options,  # noqa: F401
                    two_view_frames)
 from .features import frame_features  # noqa: F401
+from .constraints import ConstraintSettings, generate_view_constraints  # noqa: F401
 
 __version__ = "0.1.0"

@@ -1,8 +1,8 @@
 """ctypes binding of cv_b200/libcvb200.so (the C ABI declared in include/cvb200.h, cvb200_sfm.h and cvb200_tri.h) and of its modules
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
 (include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
-cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h) and cv_b200/libcvb200_init.so
-(include/cvb200_init.h)."""
+cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
+(include/cvb200_init.h) and cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h)."""
 import ctypes as C
 import os
 
@@ -119,6 +119,13 @@ ARRSAC_BATCH_MAX = 64
 # every symbol include/cvb200_init.h declares (cv-sfm's three-view initialisation), exported by libcvb200_init.so; checked by
 # tests/test_abi_init.py
 INIT_ABI_SYMBOLS = ["cvb_init_cfg_default", "cvb_init_reconstruction_dev"]
+
+# every symbol include/cvb200_constraints.h declares (cv-sfm's three-view constraints), exported by libcvb200_constraints.so; checked by
+# tests/test_abi_constraints.py
+CONSTRAINTS_ABI_SYMBOLS = ["cvb_constraints_cfg_default", "cvb_view_constraints_check", "cvb_view_constraints_dev", "cvb_view_constraints",
+                           "cvb_three_view_adaptive_optimize_l2_dev"]
+# CVB_CONSTRAINTS_MAX_LANDMARKS of include/cvb200_constraints.h
+CONSTRAINTS_MAX_LANDMARKS = 512
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -348,6 +355,34 @@ def load_init_library():
         L.cvb_init_reconstruction_dev.argtypes = [vp, vp, vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
         _INIT_LIB = L
     return _INIT_LIB
+
+
+_CONSTRAINTS_LIB = None
+
+
+def constraints_lib_path():
+    return os.path.join(_HERE, "libcvb200_constraints.so")
+
+
+def load_constraints_library():
+    """Loads libcvb200_constraints.so, the module of include/cvb200_constraints.h over libcvb200.so (same contexts). Fails loudly when
+    missing."""
+    global _CONSTRAINTS_LIB
+    if _CONSTRAINTS_LIB is None:
+        load_library()
+        p = constraints_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_constraints_cfg_default.argtypes = [vp]
+        L.cvb_constraints_cfg_default.restype = None
+        L.cvb_view_constraints_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32]
+        L.cvb_view_constraints_dev.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, u32, vp, vp, vp]
+        L.cvb_view_constraints.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u32, vp, vp, vp]
+        L.cvb_three_view_adaptive_optimize_l2_dev.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
+        _CONSTRAINTS_LIB = L
+    return _CONSTRAINTS_LIB
 
 
 class Context:

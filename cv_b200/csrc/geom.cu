@@ -19,6 +19,7 @@
 #include "../../include/cvb200_pinhole.h"
 #include "../../include/cvb200_batch.h"
 #include "../../include/cvb200_init.h"
+#include "../../include/cvb200_constraints.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1057,6 +1058,37 @@ __global__ void __launch_bounds__(OPT_NT) k_single_view_opt(const cvb_pose *__re
     if (threadIdx.x == 0) { poses_out[b] = P; updates_out[b] = updates; }
 }
 
+// The step of three_view_optimizer.rs:126-272 on the summed gradients acc = [first.t, first.r, second.t, second.r] and, adaptive, their
+// norms [first.t, first.r, second.t, second.r]; P: the inverted poses, updated in place.  Returns whether the optimisation stops.
+// k_three_view_opt's thread 0 and k_three_view_opt_warp's lane 0 both take it.
+__device__ __forceinline__ bool three_view_opt_step(const double *acc, double inv_len, int adaptive, double rate, double (&best)[2][2],
+                                                    uint32_t &no_improve, cvb_pose *P, uint32_t &updates, bool last) {
+    double d[12];
+    if (!adaptive) {
+        const double sc = inv_len * rate;
+        for (int k = 0; k < 12; k++) d[k] = acc[k] * sc;
+        no_improve++;
+        for (int v = 0; v < 2; v++) {
+            const double t = norm3(acc + 6 * v), r = norm3(acc + 6 * v + 3);
+            if (best[v][0] > t) { best[v][0] = t; no_improve = 0; }
+            if (best[v][1] > r) { best[v][1] = r; no_improve = 0; }
+        }
+        if (no_improve >= 50) return true;
+    } else {
+        for (int v = 0; v < 2; v++) {
+            double l2[6];
+            for (int k = 0; k < 6; k++) l2[k] = acc[6 * v + k] * inv_len;
+            const double tstd = acc[12 + 2 * v] * inv_len, rstd = acc[13 + 2 * v] * inv_len;
+            double trate = norm3(l2) / tstd, rrate = norm3(l2 + 3) / rstd;
+            if (!isfinite(trate)) trate = 0.0;
+            if (!isfinite(rrate)) rrate = 0.0;
+            for (int k = 0; k < 3; k++) { d[6 * v + k] = l2[k] * trate; d[6 * v + 3 + k] = l2[3 + k] * rrate; }
+        }
+    }
+    apply_delta(d, d + 3, &P[0]); apply_delta(d + 6, d + 9, &P[1]); updates++;
+    return last;
+}
+
 // three_view_optimizer.rs:126-272, one CTA per (pose pair, observation triples); obs = [centre, first, second] bearings
 __global__ void __launch_bounds__(OPT_NT) k_three_view_opt(const cvb_pose *__restrict__ poses_in, const double *__restrict__ obs,
                                                            const uint32_t *__restrict__ offsets, int adaptive, double rate,
@@ -1088,40 +1120,68 @@ __global__ void __launch_bounds__(OPT_NT) k_three_view_opt(const cvb_pose *__res
                 if (adaptive) { acc[12] += norm3(g); acc[13] += norm3(g + 3); acc[14] += norm3(g + 6); acc[15] += norm3(g + 9); }
             }
             block_sum<16>(acc, s_red);
-            if (threadIdx.x == 0) {
-                double d[12];
-                bool stop = false;
-                if (!adaptive) {
-                    const double sc = inv_len * rate;
-                    for (int k = 0; k < 12; k++) d[k] = acc[k] * sc;
-                    no_improve++;
-                    for (int v = 0; v < 2; v++) {
-                        const double t = norm3(acc + 6 * v), r = norm3(acc + 6 * v + 3);
-                        if (best[v][0] > t) { best[v][0] = t; no_improve = 0; }
-                        if (best[v][1] > r) { best[v][1] = r; no_improve = 0; }
-                    }
-                    stop = no_improve >= 50;
-                } else {
-                    for (int v = 0; v < 2; v++) {
-                        double l2[6];
-                        for (int k = 0; k < 6; k++) l2[k] = acc[6 * v + k] * inv_len;
-                        const double tstd = acc[12 + 2 * v] * inv_len, rstd = acc[13 + 2 * v] * inv_len;
-                        double trate = norm3(l2) / tstd, rrate = norm3(l2 + 3) / rstd;
-                        if (!isfinite(trate)) trate = 0.0;
-                        if (!isfinite(rrate)) rrate = 0.0;
-                        for (int k = 0; k < 3; k++) { d[6 * v + k] = l2[k] * trate; d[6 * v + 3 + k] = l2[3 + k] * rrate; }
-                    }
-                }
-                if (stop) s_stop = 1;
-                else {
-                    apply_delta(d, d + 3, &P[0]); apply_delta(d + 6, d + 9, &P[1]); updates++;
-                    if (it == iterations - 1) s_stop = 1;
-                }
-            }
+            if (threadIdx.x == 0 && three_view_opt_step(acc, inv_len, adaptive, rate, best, no_improve, P, updates, it == iterations - 1))
+                s_stop = 1;
             __syncthreads();
             if (s_stop) break;
         }
     if (threadIdx.x == 0) {
+        if (n > 0) { pose_inverse(P[0], &poses_out[2 * b]); pose_inverse(P[1], &poses_out[2 * b + 1]); }
+        else { poses_out[2 * b] = poses_in[2 * b]; poses_out[2 * b + 1] = poses_in[2 * b + 1]; }
+        updates_out[b] = updates;
+    }
+}
+
+// three_view_optimizer.rs:203-272 (adaptive), one WARP per problem of at most OPT_NT landmarks.  Lane l evaluates landmark 32 r + l of
+// row r, each row goes through block_sum's shuffle tree and lane 0 adds the row sums in row order, then +0.0 once for the rows that do not
+// exist: exactly k_three_view_opt's sums (a row is one of its warps; its idle threads and warps add +0.0), so the two agree bit for bit.
+constexpr int OPTW_NT = 128, OPTW_WARPS = OPTW_NT / 32;
+__global__ void __launch_bounds__(OPTW_NT) k_three_view_opt_warp(const cvb_pose *__restrict__ poses_in, const double *__restrict__ obs,
+                                                                 const uint32_t *__restrict__ offsets, uint32_t B, uint32_t iterations,
+                                                                 cvb_pose *__restrict__ poses_out, uint32_t *__restrict__ updates_out) {
+    __shared__ cvb_pose s_P[OPTW_WARPS][2];
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5, b = blockIdx.x * OPTW_WARPS + w;
+    if (b >= B) return;
+    const uint32_t o0 = offsets[b], n = offsets[b + 1] - o0, rows = (n + 31) / 32;
+    cvb_pose *P = s_P[w];
+    if (lane == 0 && n > 0) { pose_inverse(poses_in[2 * b], &P[0]); pose_inverse(poses_in[2 * b + 1], &P[1]); }
+    __syncwarp();
+    double best[2][2] = {{INFINITY, INFINITY}, {INFINITY, INFINITY}};
+    uint32_t no_improve = 0, updates = 0;
+    const double inv_len = 1.0 / (double)n;
+    if (n > 0)
+        for (uint32_t it = 0; it < iterations; it++) {
+            const cvb_pose P0 = P[0], P1 = P[1];
+            double tot[16];
+            for (uint32_t r = 0; r < rows; r++) {
+                double acc[16], g[12];
+                for (int k = 0; k < 16; k++) acc[k] = 0.0;
+                const uint32_t i = 32 * r + lane;
+                if (i < n) {
+                    const double *o = obs + 9 * (size_t)(o0 + i);
+                    double f[3], s[3];
+                    rotv(P0.r, o + 3, f); rotv(P1.r, o + 6, s);
+                    three_view_gradients(o, f, P0.t, s, P1.t, g);
+                    for (int k = 0; k < 12; k++) acc[k] += g[k];
+                    acc[12] += norm3(g); acc[13] += norm3(g + 3); acc[14] += norm3(g + 6); acc[15] += norm3(g + 9);
+                }
+#pragma unroll
+                for (int k = 0; k < 16; k++)
+#pragma unroll
+                    for (int o = 16; o; o >>= 1) acc[k] += __shfl_down_sync(0xffffffffu, acc[k], o);
+                for (int k = 0; k < 16; k++) tot[k] = r == 0 ? acc[k] : tot[k] + acc[k];
+            }
+            int stop = 0;
+            if (lane == 0) {
+                if (rows < (uint32_t)OPT_WARPS)
+                    for (int k = 0; k < 16; k++) tot[k] = __dadd_rn(tot[k], 0.0);
+                stop = three_view_opt_step(tot, inv_len, 1, 0.0, best, no_improve, P, updates, it == iterations - 1);
+            }
+            stop = __shfl_sync(0xffffffffu, stop, 0);
+            __syncwarp();
+            if (stop) break;
+        }
+    if (lane == 0) {
         if (n > 0) { pose_inverse(P[0], &poses_out[2 * b]); pose_inverse(P[1], &poses_out[2 * b + 1]); }
         else { poses_out[2 * b] = poses_in[2 * b]; poses_out[2 * b + 1] = poses_in[2 * b + 1]; }
         updates_out[b] = updates;
@@ -1511,6 +1571,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 }
 
 #include "init_dev.cuh"
+#include "constraints_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1669,11 +1730,13 @@ struct ArsWorkspace {
 struct GeomWorkspace {
     DevBuf a, b, samples, poses, nposes, out, masks, offsets, ok;
     DevBuf init;                    // the three-view initialisation's per-call workspace (init_reconstruction_dev)
+    DevBuf con, con2;               // the view constraints' snapshot / per-chunk and per-sub-chunk workspaces (view_constraints_dev)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
-    DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init};
+    DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
+                      &g->con2};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -2760,6 +2823,320 @@ int init_reconstruction_dev(cvb_ctx *ctx, const cvb_init_cfg *cfg, const cvb_tri
                                          combined_dev, first_matches_dev, second_matches_dev);
         CVB_LAUNCH_CHECK(ctx);
     }
+    return 0;
+}
+
+// ---- cv-sfm's three-view constraints (C names in constraints_abi.cu, include/cvb200_constraints.h; kernels in constraints_dev.cuh) ------
+void constraints_cfg_default(cvb_constraints_cfg *c) {
+    if (!c) return;
+    memset(c, 0, sizeof(*c));
+    c->robust_observation_incidence_minimum_cosine_distance = 1e-3;
+    c->robust_view_bearing_pair_minimum_cosine_distance = 1e-2;
+    c->robust_minimum_observations = 3;
+    c->robust_view_num_robust_bearing_pair = 3;
+    c->optimization_robust_covisibility_minimum_landmarks = 1u << 4;
+    c->optimization_minimum_landmarks = 24;
+    c->optimization_maximum_landmarks = 64;
+    c->optimization_maximum_three_view_constraints = 1u << 6;
+    c->optimization_minimum_new_constraints = 4;
+    c->constraint_patience = 1u << 12;
+}
+
+int three_view_adaptive_optimize_l2_dev(cvb_ctx *ctx, const cvb_pose *poses_dev, uint32_t B, const double *obs_dev, const uint32_t *offsets_dev,
+                                        uint32_t iterations, cvb_pose *poses_out_dev, uint32_t *updates_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (B == 0) return 0;
+    if (!poses_dev || !obs_dev || !offsets_dev || !poses_out_dev || !updates_dev) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    std::vector<uint32_t> off(B + 1);
+    CVB_CUDA(ctx, cudaMemcpyAsync(off.data(), offsets_dev, sizeof(uint32_t) * (B + 1), cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    for (uint32_t b = 0; b < B; b++) {
+        if (off[b + 1] < off[b]) return cvb_set_error(ctx, CVB_EINVAL, "offsets decrease at problem %u", b);
+        if (off[b + 1] - off[b] > CVB_CONSTRAINTS_MAX_LANDMARKS)
+            return cvb_set_error(ctx, CVB_EUNSUPPORTED, "problem %u: %u landmarks, at most %u", b, off[b + 1] - off[b], CVB_CONSTRAINTS_MAX_LANDMARKS);
+    }
+    {
+        CVB_PROF(ctx, "k_three_view_opt_warp", 0.0);
+        k_three_view_opt_warp<<<cdiv(B, OPTW_WARPS), OPTW_NT, 0, ctx->stream>>>(poses_dev, obs_dev, offsets_dev, B, iterations, poses_out_dev,
+                                                                              updates_dev);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+static uint32_t con_pow2(uint64_t x) { uint32_t n = 1; while (n < x) n <<= 1; return n; }
+static size_t con_align(size_t x) { return (x + 255) & ~(size_t)255; }
+// the per-chunk workspace is kept below this; a query that alone exceeds it runs alone
+constexpr size_t CON_CHUNK_BYTES = (size_t)256 << 20;
+
+int view_constraints_dev(cvb_ctx *ctx, const cvb_constraints_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                         const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, uint32_t n_features, uint32_t L,
+                         const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs, const uint32_t *queries, uint32_t Q,
+                         cvb_view_constraint *out_dev, cvb_view_constraints_result *res_dev, cvb_view_constraints_stats *stats_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses_dev || !view_off_dev || !lm_off_dev || !res_dev || (Q && !queries) || (n_features && (!view_lm_dev || !bear_dev)) ||
+        (n_obs && !obs_dev) || (Q && cfg->optimization_maximum_three_view_constraints && !out_dev))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: the constraints take a TriangulatorObservations (methods 0-2)", tri->method);
+    if (cfg->optimization_maximum_landmarks > CVB_CONSTRAINTS_MAX_LANDMARKS)
+        return cvb_set_error(ctx, CVB_EUNSUPPORTED, "optimization_maximum_landmarks %u: at most %u", cfg->optimization_maximum_landmarks,
+                             CVB_CONSTRAINTS_MAX_LANDMARKS);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    for (uint32_t i = 0; i < Q; i++)
+        if (queries[i] >= V) return cvb_set_error(ctx, CVB_EINVAL, "query %u: view %u of %u", i, queries[i], V);
+    if (Q == 0) return 0;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int sms = 0;
+    CVB_CUDA(ctx, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
+    cudaStream_t st = ctx->stream;
+    std::vector<uint32_t> vo(V + 1);
+    CVB_CUDA(ctx, cudaMemcpyAsync(vo.data(), view_off_dev, sizeof(uint32_t) * (V + 1), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (vo[V] != n_features) return cvb_set_error(ctx, CVB_EINVAL, "view_offsets[V] = %u, n_features %u", vo[V], n_features);
+    ConParams prm;
+    prm.inc = cfg->robust_observation_incidence_minimum_cosine_distance;
+    prm.bp_min_cos = cfg->robust_view_bearing_pair_minimum_cosine_distance;
+    prm.V = V;
+    prm.min_obs = std::min(cfg->robust_minimum_observations, V);
+    prm.covis_min = cfg->optimization_robust_covisibility_minimum_landmarks;
+    prm.opt_min = cfg->optimization_minimum_landmarks;
+    prm.opt_max = cfg->optimization_maximum_landmarks;
+    prm.bp_min = cfg->robust_view_num_robust_bearing_pair;
+    prm.max_c = cfg->optimization_maximum_three_view_constraints;
+    prm.min_new = cfg->optimization_minimum_new_constraints;
+    const cvb_triangulator T = *tri;
+    const uint32_t maxc = prm.max_c, omax = std::max<uint32_t>(prm.opt_max, 1), vw = (V + 31) / 32;
+    // per chunk query: robust list, three V-sized arrays, its ConQuery
+    auto bytes_a = [&](uint32_t q) { return sizeof(uint32_t) * ((size_t)(vo[q + 1] - vo[q]) + 3 * (size_t)V) + sizeof(ConQuery); };
+    size_t chunk_a = 0, cur = 0;
+    for (uint32_t i = 0; i < Q; i++) {
+        const size_t b = bytes_a(queries[i]);
+        if (cur && cur + b > CON_CHUNK_BYTES) { chunk_a = std::max(chunk_a, cur); cur = 0; }
+        cur += b;
+    }
+    chunk_a = std::max(chunk_a, cur) + 8 * 256;
+    // snapshot part: per observation pose, bearing, world bearing (and SineL1's scratch), per landmark the robust flag; then the chunk part
+    size_t off = 0;
+    const size_t o_pose = off; off += con_align(sizeof(cvb_pose) * (size_t)n_obs);
+    const size_t o_bear = off; off += con_align(sizeof(double) * 3 * (size_t)n_obs);
+    const size_t o_world = off; off += con_align(sizeof(double) * 3 * (size_t)n_obs);
+    const size_t o_W = off; off += tri->method == CVB_TRI_SINE_L1 ? con_align(sizeof(double) * 6 * (size_t)n_obs) : 0;
+    const size_t o_rob = off; off += con_align(L);
+    const size_t o_chunk = off; off += chunk_a;
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->con.ensure(ctx, off))) return rc;
+    unsigned char *base = (unsigned char *)g->con.p;
+    cvb_pose *obs_pose = (cvb_pose *)(base + o_pose);
+    double *obs_bear = (double *)(base + o_bear), *obs_world = (double *)(base + o_world);
+    double *W = tri->method == CVB_TRI_SINE_L1 ? (double *)(base + o_W) : nullptr;
+    uint8_t *robust = base + o_rob;
+    if (n_obs) {
+        CVB_PROF(ctx, "k_con_gather_obs", 0);
+        k_con_gather_obs<<<cdiv(n_obs, 256), 256, 0, st>>>(poses_dev, view_off_dev, bear_dev, obs_dev, n_obs, obs_pose, obs_bear, obs_world);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (L) {
+        CVB_PROF(ctx, "k_con_robust", 0);
+        k_con_robust<<<cdiv(L, 128), 128, 0, st>>>(T, lm_off_dev, L, obs_pose, obs_bear, obs_world, W, prm, robust);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    std::vector<ConQuery> hq;
+    for (uint32_t c0 = 0; c0 < Q;) {
+        // chunk [c0, c1): phase A
+        uint32_t c1 = c0;
+        size_t used = 0, nrl = 0;
+        while (c1 < Q && (c1 == c0 || used + bytes_a(queries[c1]) <= CON_CHUNK_BYTES)) { used += bytes_a(queries[c1]); nrl += vo[queries[c1] + 1] - vo[queries[c1]]; c1++; }
+        const uint32_t Qc = c1 - c0;
+        unsigned char *cb = base + o_chunk;
+        size_t co = 0;
+        ConQuery *qs = (ConQuery *)(cb + co); co += con_align(sizeof(ConQuery) * Qc);
+        uint32_t *cnt = (uint32_t *)(cb + co); co += con_align(sizeof(uint32_t) * (size_t)Qc * V);
+        uint32_t *kidx = (uint32_t *)(cb + co); co += con_align(sizeof(uint32_t) * (size_t)Qc * V);
+        uint32_t *kview = (uint32_t *)(cb + co); co += con_align(sizeof(uint32_t) * (size_t)Qc * V);
+        uint32_t *rlist = (uint32_t *)(cb + co); co += con_align(sizeof(uint32_t) * std::max<size_t>(nrl, 1));
+        hq.assign(Qc, ConQuery());
+        uint32_t rb = 0;
+        for (uint32_t j = 0; j < Qc; j++) {
+            memset(&hq[j], 0, sizeof(ConQuery));
+            hq[j].q = queries[c0 + j]; hq[j].out = c0 + j; hq[j].rbase = rb;
+            rb += vo[hq[j].q + 1] - vo[hq[j].q];
+        }
+        CVB_CUDA(ctx, cudaMemcpyAsync(qs, hq.data(), sizeof(ConQuery) * Qc, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * (size_t)Qc * V, st));
+        {
+            CVB_PROF(ctx, "k_con_lists", 0);
+            k_con_lists<<<Qc, 256, 0, st>>>(view_off_dev, view_lm_dev, lm_off_dev, obs_dev, robust, prm, qs, rlist, cnt, kidx, kview);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        CVB_CUDA(ctx, cudaMemcpyAsync(hq.data(), qs, sizeof(ConQuery) * Qc, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        // phase B over sub-chunks [s0, s1) of the chunk
+        auto bytes_b = [&](const ConQuery &q) {
+            const uint64_t P = (uint64_t)q.K * (q.K - (q.K > 0)) / 2;
+            return sizeof(uint32_t) * ((size_t)q.K * ((q.R + 31) / 32) + 2 * P + vw) + sizeof(unsigned long long) * (con_pow2(P) + con_pow2(q.R)) +
+                   (size_t)maxc * (2 * sizeof(double) * 9 * omax + 4 * sizeof(cvb_pose) + sizeof(uint32_t) * 6 + sizeof(double)) + 16 * 256;
+        };
+        for (uint32_t s0 = 0; s0 < Qc;) {
+            uint32_t s1 = s0;
+            size_t ub = 0;
+            while (s1 < Qc && (s1 == s0 || ub + bytes_b(hq[s1]) <= CON_CHUNK_BYTES)) ub += bytes_b(hq[s1++]);
+            const uint32_t Qs = s1 - s0, B = Qs * maxc;
+            uint32_t nb = 0, nk = 0, npair = 0, nsort = 0, max_n2 = 1;
+            for (uint32_t j = s0; j < s1; j++) {
+                ConQuery &q = hq[j];
+                const uint64_t P = (uint64_t)q.K * (q.K - (q.K > 0)) / 2;
+                if (P >= (1ull << 31)) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "query %u: %u coviews", q.out, q.K);
+                q.words = (q.R + 31) / 32; q.bbase = nb; nb += q.K * q.words;
+                q.P = (uint32_t)P; q.n2 = con_pow2(P); q.kbase = nk; nk += q.n2; q.obase = npair; npair += q.P;
+                q.s2 = con_pow2(q.R); q.sbase = nsort; nsort += q.s2;
+                max_n2 = std::max(max_n2, q.n2);
+            }
+            size_t bo = 0;
+            const size_t b_bits = bo; bo += con_align(sizeof(uint32_t) * std::max<uint32_t>(nb, 1));
+            const size_t b_keys = bo; bo += con_align(sizeof(unsigned long long) * nk);
+            const size_t b_pcnt = bo; bo += con_align(sizeof(uint32_t) * std::max<uint32_t>(npair, 1));
+            const size_t b_ord = bo; bo += con_align(sizeof(uint32_t) * std::max<uint32_t>(npair, 1));
+            const size_t b_vis = bo; bo += con_align(sizeof(uint32_t) * (size_t)Qs * vw);
+            const size_t b_sort = bo; bo += con_align(sizeof(unsigned long long) * nsort);
+            const size_t b_rows = bo; bo += con_align(sizeof(double) * 9 * (size_t)std::max<uint32_t>(B, 1) * omax);
+            const size_t b_pack = bo; bo += con_align(sizeof(double) * 9 * (size_t)std::max<uint32_t>(B, 1) * omax);
+            const size_t b_pin = bo; bo += con_align(sizeof(cvb_pose) * 2 * (size_t)std::max<uint32_t>(B, 1));
+            const size_t b_pout = bo; bo += con_align(sizeof(cvb_pose) * 2 * (size_t)std::max<uint32_t>(B, 1));
+            const size_t b_pn = bo; bo += con_align(sizeof(uint32_t) * std::max<uint32_t>(B, 1));
+            const size_t b_pv = bo; bo += con_align(sizeof(uint32_t) * 3 * (size_t)std::max<uint32_t>(B, 1));
+            const size_t b_ps = bo; bo += con_align(sizeof(double) * std::max<uint32_t>(B, 1));
+            const size_t b_off = bo; bo += con_align(sizeof(uint32_t) * (B + 1));
+            const size_t b_upd = bo; bo += con_align(sizeof(uint32_t) * std::max<uint32_t>(B, 1));
+            if ((rc = g->con2.ensure(ctx, bo))) return rc;
+            unsigned char *sb = (unsigned char *)g->con2.p;
+            uint32_t *bits = (uint32_t *)(sb + b_bits), *pcnt = (uint32_t *)(sb + b_pcnt), *ord = (uint32_t *)(sb + b_ord);
+            uint32_t *vis = (uint32_t *)(sb + b_vis), *pn = (uint32_t *)(sb + b_pn), *pv = (uint32_t *)(sb + b_pv);
+            uint32_t *poff = (uint32_t *)(sb + b_off), *upd = (uint32_t *)(sb + b_upd);
+            unsigned long long *keys = (unsigned long long *)(sb + b_keys), *sortbuf = (unsigned long long *)(sb + b_sort);
+            double *rows = (double *)(sb + b_rows), *packed = (double *)(sb + b_pack), *ps = (double *)(sb + b_ps);
+            cvb_pose *pin = (cvb_pose *)(sb + b_pin), *pout = (cvb_pose *)(sb + b_pout);
+            ConQuery *qsub = qs + s0;
+            uint32_t *ki = kidx + (size_t)s0 * V, *kv = kview + (size_t)s0 * V;
+            CVB_CUDA(ctx, cudaMemcpyAsync(qsub, hq.data() + s0, sizeof(ConQuery) * Qs, cudaMemcpyHostToDevice, st));
+            CVB_CUDA(ctx, cudaMemsetAsync(bits, 0, sizeof(uint32_t) * std::max<uint32_t>(nb, 1), st));
+            CVB_CUDA(ctx, cudaMemsetAsync(vis, 0, sizeof(uint32_t) * (size_t)Qs * vw, st));
+            {
+                CVB_PROF(ctx, "k_con_triples", 0);
+                k_con_bits<<<Qs, 256, 0, st>>>(lm_off_dev, obs_dev, prm, qsub, rlist, ki, bits);
+                CVB_LAUNCH_CHECK(ctx);
+                k_con_pairs<<<dim3(cdiv(max_n2, 8), Qs), 256, 0, st>>>(prm, qsub, bits, keys, pcnt);
+                CVB_LAUNCH_CHECK(ctx);
+                k_con_order<<<Qs, 1024, 0, st>>>(prm, qsub, kv, keys, vis, ord);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            {
+                CVB_PROF(ctx, "k_con_select", 0);
+                k_con_select<<<Qs, 256, 0, st>>>(poses_dev, view_off_dev, bear_dev, lm_off_dev, obs_dev, prm, qsub, rlist, kv, bits, keys, pcnt,
+                                                 ord, sortbuf, rows, pin, pn, pv, ps);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            if (B) {
+                {
+                    CVB_PROF(ctx, "k_con_pack", 0);
+                    k_con_offsets<<<1, 32, 0, st>>>(B, pn, poff);
+                    CVB_LAUNCH_CHECK(ctx);
+                    k_con_pack<<<B, 256, 0, st>>>(omax, pn, poff, rows, packed);
+                    CVB_LAUNCH_CHECK(ctx);
+                }
+                // The two kernels give the same bits (tests/test_gpu_constraints.py).  A batch that fits one CTA per SM (one query) runs
+                // faster on k_three_view_opt's 512 threads per problem; a larger one on k_three_view_opt_warp's eight problems per SM
+                // (DESIGN section 4l).
+                if (B <= (uint32_t)sms) {
+                    CVB_PROF(ctx, "k_three_view_opt", 0);
+                    k_three_view_opt<<<B, OPT_NT, 0, st>>>(pin, packed, poff, 1, 0.0, cfg->constraint_patience, pout, upd);
+                    CVB_LAUNCH_CHECK(ctx);
+                } else {
+                    CVB_PROF(ctx, "k_three_view_opt_warp", 0);
+                    k_three_view_opt_warp<<<cdiv(B, OPTW_WARPS), OPTW_NT, 0, st>>>(pin, packed, poff, B, cfg->constraint_patience, pout, upd);
+                    CVB_LAUNCH_CHECK(ctx);
+                }
+            }
+            {
+                CVB_PROF(ctx, "k_con_finish", 0);
+                k_con_finish<<<Qs, 64, 0, st>>>(prm, qsub, pout, upd, pn, pv, ps, out_dev, res_dev, stats_dev);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            s0 = s1;
+        }
+        c0 = c1;
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int view_constraints_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                           const uint32_t *queries, uint32_t Q) {
+    if (!vo || !lo || (Q && !queries)) return CVB_EINVAL;
+    if (V == 0 || vo[0] != 0 || lo[0] != 0) return CVB_EINVAL;
+    for (uint32_t v = 0; v < V; v++) if (vo[v + 1] < vo[v]) return CVB_EINVAL;
+    for (uint32_t l = 0; l < L; l++) if (lo[l + 1] < lo[l]) return CVB_EINVAL;
+    if ((vo[V] && !vl) || (lo[L] && !obs)) return CVB_EINVAL;
+    for (uint32_t i = 0; i < Q; i++) if (queries[i] >= V) return CVB_EINVAL;
+    for (uint32_t f = 0; f < vo[V]; f++) if (vl[f] >= L) return CVB_EINVAL;
+    // every observation names an existing feature of its view, that feature names the landmark back, and no view is observed twice;
+    // with as many observations as features, that makes the two CSRs each other's inverse
+    if (lo[L] != vo[V]) return CVB_EINVAL;
+    std::vector<uint32_t> last(V, 0xffffffffu);
+    for (uint32_t l = 0; l < L; l++)
+        for (uint32_t o = lo[l]; o < lo[l + 1]; o++) {
+            const uint32_t v = obs[2 * (size_t)o], f = obs[2 * (size_t)o + 1];
+            if (v >= V || f >= vo[v + 1] - vo[v] || vl[vo[v] + f] != l || last[v] == l) return CVB_EINVAL;
+            last[v] = l;
+        }
+    return 0;
+}
+
+int view_constraints(cvb_ctx *ctx, const cvb_constraints_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                     const uint32_t *vo, const uint32_t *vl, const double *bear, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                     const uint32_t *queries, uint32_t Q, cvb_view_constraint *out, cvb_view_constraints_result *res,
+                     cvb_view_constraints_stats *stats) {
+    if (!ctx) return CVB_EINVAL;
+    const uint32_t maxc = cfg ? cfg->optimization_maximum_three_view_constraints : 0;
+    if (!cfg || !tri || !poses || !res || (Q && maxc && !out)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (view_constraints_check(V, vo, vl, L, lo, obs, queries, Q)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot or queries");
+    if (vo[V] && !bear) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    const uint32_t nf = vo[V], no = lo[L];
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    size_t off = 0;
+    const size_t i_pose = off; off += con_align(sizeof(cvb_pose) * V);
+    const size_t i_vo = off; off += con_align(sizeof(uint32_t) * (V + 1));
+    const size_t i_vl = off; off += con_align(sizeof(uint32_t) * (size_t)nf);
+    const size_t i_bear = off; off += con_align(sizeof(double) * 3 * (size_t)nf);
+    const size_t i_lo = off; off += con_align(sizeof(uint32_t) * ((size_t)L + 1));
+    const size_t i_obs = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)no);
+    const size_t i_out = off; off += con_align(sizeof(cvb_view_constraint) * (size_t)Q * maxc);
+    const size_t i_res = off; off += con_align(sizeof(cvb_view_constraints_result) * (size_t)Q);
+    const size_t i_st = off; off += con_align(sizeof(cvb_view_constraints_stats) * (size_t)Q);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->out.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->out.p;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_pose, poses, sizeof(cvb_pose) * V, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_vo, vo, sizeof(uint32_t) * (V + 1), cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_vl, vl, sizeof(uint32_t) * (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_bear, bear, sizeof(double) * 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_lo, lo, sizeof(uint32_t) * ((size_t)L + 1), cudaMemcpyHostToDevice, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_obs, obs, sizeof(uint32_t) * 2 * (size_t)no, cudaMemcpyHostToDevice, st));
+    if ((rc = view_constraints_dev(ctx, cfg, tri, V, (const cvb_pose *)(b + i_pose), (const uint32_t *)(b + i_vo), (const uint32_t *)(b + i_vl),
+                                   (const double *)(b + i_bear), nf, L, (const uint32_t *)(b + i_lo), (const uint32_t *)(b + i_obs), no, queries,
+                                   Q, (cvb_view_constraint *)(b + i_out), (cvb_view_constraints_result *)(b + i_res),
+                                   stats ? (cvb_view_constraints_stats *)(b + i_st) : nullptr)))
+        return rc;
+    if (Q && maxc) CVB_CUDA(ctx, cudaMemcpyAsync(out, b + i_out, sizeof(cvb_view_constraint) * (size_t)Q * maxc, cudaMemcpyDeviceToHost, st));
+    if (Q) CVB_CUDA(ctx, cudaMemcpyAsync(res, b + i_res, sizeof(cvb_view_constraints_result) * (size_t)Q, cudaMemcpyDeviceToHost, st));
+    if (Q && stats) CVB_CUDA(ctx, cudaMemcpyAsync(stats, b + i_st, sizeof(cvb_view_constraints_stats) * (size_t)Q, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
 
