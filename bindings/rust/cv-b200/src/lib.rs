@@ -210,3 +210,6 @@ pub mod init;
 
 // ---- INTEGRATION.md section 2m (include/cvb200_constraints.h) ----
 pub mod constraints;
+
+// ---- INTEGRATION.md section 2n (include/cvb200_reconstruction.h) ----
+pub mod reconstruction;

@@ -22,6 +22,9 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
                            three-view choice over every pair of them, chained on the device
   generate_view_constraints, ConstraintSettings <- cv-sfm VSlam::generate_view_constraints / record_view_constraints
                            (cv-sfm/src/lib.rs:2092-2109, 2438-2516) for many views of one reconstruction snapshot in one call
+  optimize_reconstruction, regenerate_reconstruction, ReconstructionSettings <- cv-sfm VSlam::optimize_reconstruction /
+                           regenerate_reconstruction (cv-sfm/src/lib.rs:2343-2435): the three-view pose graph and the observation
+                           filter of one reconstruction snapshot in one call
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -50,5 +53,6 @@ from .pair import (InitSettings, Intrinsics, IntrinsicsK1, TwoViewBuffers, init_
                    two_view_frames)
 from .features import frame_features  # noqa: F401
 from .constraints import ConstraintSettings, generate_view_constraints  # noqa: F401
+from .reconstruction import ReconstructionSettings, optimize_reconstruction, regenerate_reconstruction  # noqa: F401
 
 __version__ = "0.1.0"

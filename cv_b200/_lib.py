@@ -2,7 +2,8 @@
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
 (include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
-(include/cvb200_init.h) and cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h)."""
+(include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h) and cv_b200/libcvb200_reconstruction.so
+(include/cvb200_reconstruction.h)."""
 import ctypes as C
 import os
 
@@ -126,6 +127,11 @@ CONSTRAINTS_ABI_SYMBOLS = ["cvb_constraints_cfg_default", "cvb_view_constraints_
                            "cvb_three_view_adaptive_optimize_l2_dev"]
 # CVB_CONSTRAINTS_MAX_LANDMARKS of include/cvb200_constraints.h
 CONSTRAINTS_MAX_LANDMARKS = 512
+
+# every symbol include/cvb200_reconstruction.h declares (cv-sfm's reconstruction optimisation), exported by libcvb200_reconstruction.so;
+# checked by tests/test_abi_reconstruction.py
+RECONSTRUCTION_ABI_SYMBOLS = ["cvb_recon_cfg_default", "cvb_optimize_reconstruction_check", "cvb_optimize_reconstruction_dev",
+                              "cvb_optimize_reconstruction"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -383,6 +389,33 @@ def load_constraints_library():
         L.cvb_three_view_adaptive_optimize_l2_dev.argtypes = [vp, vp, u32, vp, vp, u32, vp, vp]
         _CONSTRAINTS_LIB = L
     return _CONSTRAINTS_LIB
+
+
+_RECONSTRUCTION_LIB = None
+
+
+def reconstruction_lib_path():
+    return os.path.join(_HERE, "libcvb200_reconstruction.so")
+
+
+def load_reconstruction_library():
+    """Loads libcvb200_reconstruction.so, the module of include/cvb200_reconstruction.h over libcvb200.so (same contexts). Fails loudly
+    when missing."""
+    global _RECONSTRUCTION_LIB
+    if _RECONSTRUCTION_LIB is None:
+        load_library()
+        p = reconstruction_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_recon_cfg_default.argtypes = [vp]
+        L.cvb_recon_cfg_default.restype = None
+        L.cvb_optimize_reconstruction_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32]
+        L.cvb_optimize_reconstruction_dev.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, u32, vp, vp, vp, vp]
+        L.cvb_optimize_reconstruction.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u32, vp, vp, vp, vp]
+        _RECONSTRUCTION_LIB = L
+    return _RECONSTRUCTION_LIB
 
 
 class Context:

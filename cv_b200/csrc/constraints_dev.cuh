@@ -51,7 +51,20 @@ __device__ __forceinline__ void con_pose_mul(const cvb_pose &A, const cvb_pose &
     for (int i = 0; i < 3; i++) o->t[i] = A.t[i] + sh[i];
 }
 
-// per observation: the view's pose, the bearing, and the world-frame bearing (pose^-1's rotation applied to it, lib.rs:2985-2988)
+// the world-frame bearing of an observation: pose^-1's rotation applied to the bearing (lib.rs:2985-2988)
+__device__ __forceinline__ void world_bearing(const cvb_pose &P, const double *b, double *o) {
+    for (int r = 0; r < 3; r++) o[r] = P.r[r] * b[0] + P.r[3 + r] * b[1] + P.r[6 + r] * b[2];
+}
+// are_observations_robust (lib.rs:2907-2934) over the n world-frame bearings world[o0 ..): at least min_obs of them, and some pair
+// i < j, in tuple_combinations order, with 1 - a.b > inc
+__device__ __forceinline__ bool observations_robust(const double *world, uint32_t o0, uint32_t n, uint32_t min_obs, double inc) {
+    bool ok = n >= min_obs, incident = false;
+    for (uint32_t i = 0; ok && !incident && i < n; i++)
+        for (uint32_t j = i + 1; !incident && j < n; j++)
+            incident = 1.0 - dot3(world + 3 * (size_t)(o0 + i), world + 3 * (size_t)(o0 + j)) > inc;
+    return ok && incident;
+}
+// per observation: the view's pose, the bearing, and the world-frame bearing
 __global__ void __launch_bounds__(256) k_con_gather_obs(const cvb_pose *__restrict__ poses, const uint32_t *__restrict__ view_off,
                                                         const double *__restrict__ bear, const uint32_t *__restrict__ obs, uint32_t n_obs,
                                                         cvb_pose *__restrict__ obs_pose, double *__restrict__ obs_bear,
@@ -62,10 +75,8 @@ __global__ void __launch_bounds__(256) k_con_gather_obs(const cvb_pose *__restri
     const cvb_pose P = poses[v];
     const double *b = bear + 3 * ((size_t)view_off[v] + f);
     obs_pose[o] = P;
-    for (int r = 0; r < 3; r++) {
-        obs_bear[3 * (size_t)o + r] = b[r];
-        obs_world[3 * (size_t)o + r] = P.r[r] * b[0] + P.r[3 + r] * b[1] + P.r[6 + r] * b[2];
-    }
+    for (int r = 0; r < 3; r++) obs_bear[3 * (size_t)o + r] = b[r];
+    world_bearing(P, b, obs_world + 3 * (size_t)o);
 }
 // triangulate_landmark_robust is Some (lib.rs:2907-2934, 2975-3000); one thread per landmark
 __global__ void __launch_bounds__(128) k_con_robust(cvb_triangulator T, const uint32_t *__restrict__ lm_off, uint32_t L,
@@ -75,11 +86,7 @@ __global__ void __launch_bounds__(128) k_con_robust(cvb_triangulator T, const ui
     const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= L) return;
     const uint32_t o0 = lm_off[l], n = lm_off[l + 1] - o0;
-    bool ok = n >= prm.min_obs, incident = false;
-    for (uint32_t i = 0; ok && !incident && i < n; i++)
-        for (uint32_t j = i + 1; !incident && j < n; j++)
-            incident = 1.0 - dot3(obs_world + 3 * (size_t)(o0 + i), obs_world + 3 * (size_t)(o0 + j)) > prm.inc;
-    ok = ok && incident;
+    bool ok = observations_robust(obs_world, o0, n, prm.min_obs, prm.inc);
     if (ok) {
         double p[4];
         ok = triangulate_observations(T, obs_pose + o0, obs_bear + 3 * (size_t)o0, n, W ? W + 6 * (size_t)o0 : nullptr, p);

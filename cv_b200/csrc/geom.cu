@@ -13,6 +13,7 @@
 #include <string.h>
 #include <algorithm>
 #include <vector>
+#include <cooperative_groups.h>
 #include "common.cuh"
 #include "../../include/cvb200_tri.h"
 #include "../../include/cvb200_opt.h"
@@ -20,6 +21,7 @@
 #include "../../include/cvb200_batch.h"
 #include "../../include/cvb200_init.h"
 #include "../../include/cvb200_constraints.h"
+#include "../../include/cvb200_reconstruction.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1572,6 +1574,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 
 #include "init_dev.cuh"
 #include "constraints_dev.cuh"
+#include "reconstruction_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1731,12 +1734,13 @@ struct GeomWorkspace {
     DevBuf a, b, samples, poses, nposes, out, masks, offsets, ok;
     DevBuf init;                    // the three-view initialisation's per-call workspace (init_reconstruction_dev)
     DevBuf con, con2;               // the view constraints' snapshot / per-chunk and per-sub-chunk workspaces (view_constraints_dev)
+    DevBuf rec;                     // the reconstruction optimisation's workspace (optimize_reconstruction_dev)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2};
+                      &g->con2, &g->rec};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -3136,6 +3140,193 @@ int view_constraints(cvb_ctx *ctx, const cvb_constraints_cfg *cfg, const cvb_tri
     if (Q && maxc) CVB_CUDA(ctx, cudaMemcpyAsync(out, b + i_out, sizeof(cvb_view_constraint) * (size_t)Q * maxc, cudaMemcpyDeviceToHost, st));
     if (Q) CVB_CUDA(ctx, cudaMemcpyAsync(res, b + i_res, sizeof(cvb_view_constraints_result) * (size_t)Q, cudaMemcpyDeviceToHost, st));
     if (Q && stats) CVB_CUDA(ctx, cudaMemcpyAsync(stats, b + i_st, sizeof(cvb_view_constraints_stats) * (size_t)Q, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+// ---- cv-sfm's reconstruction optimisation (C names in reconstruction_abi.cu, include/cvb200_reconstruction.h; kernels in
+// reconstruction_dev.cuh) -----------------------------------------------------------------------------------------------------------
+void recon_cfg_default(cvb_recon_cfg *c) {
+    if (!c) return;
+    memset(c, 0, sizeof(*c));
+    c->graph_optimization_rate = 0.001;
+    c->maximum_sine_distance = 0.1;
+    c->maximum_cosine_distance = 1e-5;
+    c->robust_observation_incidence_minimum_cosine_distance = 1e-3;
+    c->optimization_iterations = 1u << 10;
+    c->reconstruction_optimization_iterations = 1;
+    c->robust_minimum_observations = 3;
+    c->minimum_robust_landmarks = 32;
+}
+
+int optimize_reconstruction_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                                  const cvb_view_constraint *cons, uint32_t C) {
+    if (view_constraints_check(V, vo, vl, L, lo, obs, nullptr, 0)) return CVB_EINVAL;
+    if (C && !cons) return CVB_EINVAL;
+    for (uint32_t c = 0; c < C; c++) {
+        const uint32_t *w = cons[c].views;
+        if (w[0] >= V || w[1] >= V || w[2] >= V || w[0] == w[1] || w[0] == w[2] || w[1] == w[2]) return CVB_EINVAL;
+    }
+    return 0;
+}
+
+int optimize_reconstruction_dev(cvb_ctx *ctx, const cvb_recon_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                                const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, uint32_t n_features,
+                                uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs,
+                                const cvb_view_constraint *cons_dev, uint32_t C, cvb_recon_result *res_dev, cvb_pose *poses_out_dev,
+                                uint8_t *view_state_dev, uint8_t *obs_state_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses_dev || !view_off_dev || !lm_off_dev || !res_dev || !poses_out_dev || !view_state_dev ||
+        (n_features && (!view_lm_dev || !bear_dev)) || (n_obs && (!obs_dev || !obs_state_dev)) || (C && !cons_dev))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: the filter takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    uint32_t nf = 0;
+    CVB_CUDA(ctx, cudaMemcpyAsync(&nf, view_off_dev + V, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (nf != n_features) return cvb_set_error(ctx, CVB_EINVAL, "view_offsets[V] = %u, n_features %u", nf, n_features);
+    RecParams prm;
+    prm.rate = cfg->graph_optimization_rate;
+    prm.max_sin = cfg->maximum_sine_distance;
+    prm.max_cos = cfg->maximum_cosine_distance;
+    prm.inc = cfg->robust_observation_incidence_minimum_cosine_distance;
+    prm.V = V;
+    prm.C = C;
+    prm.iters = cfg->optimization_iterations;
+    prm.min_obs_cfg = cfg->robust_minimum_observations;
+    prm.min_robust = cfg->minimum_robust_landmarks;
+    const size_t E = 6 * (size_t)C;
+    size_t off = 0;
+    const size_t o_ctl = off; off += con_align(sizeof(RecCtl));
+    const size_t o_pose = off; off += con_align(sizeof(cvb_pose) * 2 * (size_t)V);
+    const size_t o_state = off; off += con_align(2 * (size_t)V);
+    const size_t o_deg = off; off += con_align(sizeof(uint32_t) * (size_t)V);
+    const size_t o_eoff = off; off += con_align(sizeof(uint32_t) * ((size_t)V + 1));
+    const size_t o_ev = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(E, 1));
+    const size_t o_eo = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(E, 1));
+    const size_t o_eT = off; off += con_align(sizeof(cvb_pose) * std::max<size_t>(E, 1));
+    const size_t o_se3 = off; off += con_align(sizeof(double) * 6 * std::max<size_t>(E, 1));
+    const size_t o_gp = off; off += con_align(sizeof(cvb_pose) * std::max<size_t>(n_obs, 1));
+    const size_t o_gb = off; off += con_align(sizeof(double) * 3 * std::max<size_t>(n_obs, 1));
+    const size_t o_gw = off; off += con_align(sizeof(double) * 3 * std::max<size_t>(n_obs, 1));
+    const size_t o_gi = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(n_obs, 1));
+    const size_t o_W = off; off += tri->method == CVB_TRI_SINE_L1 ? con_align(sizeof(double) * 6 * std::max<size_t>(n_obs, 1)) : 0;
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->rec.ensure(ctx, off))) return rc;
+    unsigned char *base = (unsigned char *)g->rec.p;
+    RecCtl *ctl = (RecCtl *)(base + o_ctl);
+    cvb_pose *pbuf = (cvb_pose *)(base + o_pose), *eT = (cvb_pose *)(base + o_eT), *gp = (cvb_pose *)(base + o_gp);
+    uint8_t *sbuf = base + o_state;
+    uint32_t *deg = (uint32_t *)(base + o_deg), *eoff = (uint32_t *)(base + o_eoff), *ev = (uint32_t *)(base + o_ev);
+    uint32_t *eo = (uint32_t *)(base + o_eo), *gi = (uint32_t *)(base + o_gi);
+    double *se3 = (double *)(base + o_se3), *gb = (double *)(base + o_gb), *gw = (double *)(base + o_gw);
+    double *W = tri->method == CVB_TRI_SINE_L1 ? (double *)(base + o_W) : nullptr;
+    int sms = 0, per_sm = 0;
+    CVB_CUDA(ctx, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device));
+    CVB_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rec_steps, REC_NT, 0));
+    if (per_sm < 1) return cvb_set_error(ctx, CVB_ECUDA, "k_rec_steps cannot be resident");
+    // every block must be resident for the grid barrier; more than the larger stage needs would only wait at it
+    const size_t need = std::max((E + REC_NT - 1) / REC_NT, ((size_t)V * 32 + REC_NT - 1) / REC_NT);
+    const uint32_t grid = (uint32_t)std::max<size_t>(1, std::min<size_t>((size_t)sms * per_sm, need));
+    const cvb_triangulator T = *tri;
+    {
+        CVB_PROF(ctx, "k_rec_init", 0);
+        k_rec_init<<<1, 1, 0, st>>>(ctl);
+        CVB_LAUNCH_CHECK(ctx);
+        CVB_CUDA(ctx, cudaMemcpyAsync(pbuf, poses_dev, sizeof(cvb_pose) * V, cudaMemcpyDeviceToDevice, st));
+        CVB_CUDA(ctx, cudaMemsetAsync(sbuf, 0, 2 * (size_t)V, st));
+        if (n_obs) CVB_CUDA(ctx, cudaMemsetAsync(obs_state_dev, 0, n_obs, st));
+    }
+    for (uint32_t r = 0; r < cfg->reconstruction_optimization_iterations; r++) {
+        {
+            CVB_PROF(ctx, "k_rec_flatten", 0);
+            CVB_CUDA(ctx, cudaMemsetAsync(deg, 0, sizeof(uint32_t) * V, st));
+            if (C) {
+                k_rec_count<<<cdiv(C, 256), 256, 0, st>>>(prm, ctl, cons_dev, sbuf, deg);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            k_rec_scan<<<1, 32, 0, st>>>(prm, ctl, deg, eoff);
+            CVB_LAUNCH_CHECK(ctx);
+            if (C) {
+                k_rec_place<<<cdiv((size_t)V * 32, 256), 256, 0, st>>>(prm, ctl, cons_dev, sbuf, eoff, ev, eo, eT);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+        }
+        if (prm.iters) {
+            CVB_PROF(ctx, "k_rec_steps", 0);
+            void *args[] = {&prm, &ctl, &eoff, &ev, &eo, &eT, &se3, &pbuf, &sbuf, &r};
+            CVB_CUDA(ctx, cudaLaunchCooperativeKernel((const void *)k_rec_steps, dim3(grid), dim3(REC_NT), args, 0, st));
+        }
+        {
+            CVB_PROF(ctx, "k_rec_filter", 0);
+            k_rec_present<<<1, 256, 0, st>>>(prm, ctl, sbuf);
+            CVB_LAUNCH_CHECK(ctx);
+            if (L) {
+                k_rec_filter<<<cdiv(L, 128), 128, 0, st>>>(T, prm, ctl, pbuf, sbuf, view_off_dev, bear_dev, lm_off_dev, obs_dev, L, obs_state_dev,
+                                                            gp, gb, gw, gi, W);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            k_rec_judge<<<1, 1, 0, st>>>(prm, ctl, r);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+    }
+    {
+        CVB_PROF(ctx, "k_rec_finish", 0);
+        k_rec_finish<<<1, 256, 0, st>>>(prm, ctl, pbuf, sbuf, cfg->reconstruction_optimization_iterations, res_dev, poses_out_dev, view_state_dev);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int optimize_reconstruction(cvb_ctx *ctx, const cvb_recon_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                            const uint32_t *vo, const uint32_t *vl, const double *bear, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                            const cvb_view_constraint *cons, uint32_t C, cvb_recon_result *res, cvb_pose *poses_out, uint8_t *view_state,
+                            uint8_t *obs_state) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses || !res || !poses_out || !view_state) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (optimize_reconstruction_check(V, vo, vl, L, lo, obs, cons, C)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot or constraints");
+    const uint32_t nf = vo[V], no = lo[L];
+    if ((nf && !bear) || (no && !obs_state)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    size_t off = 0;
+    const size_t i_pose = off; off += con_align(sizeof(cvb_pose) * V);
+    const size_t i_vo = off; off += con_align(sizeof(uint32_t) * (V + 1));
+    const size_t i_vl = off; off += con_align(sizeof(uint32_t) * (size_t)nf);
+    const size_t i_bear = off; off += con_align(sizeof(double) * 3 * (size_t)nf);
+    const size_t i_lo = off; off += con_align(sizeof(uint32_t) * ((size_t)L + 1));
+    const size_t i_obs = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)no);
+    const size_t i_cons = off; off += con_align(sizeof(cvb_view_constraint) * (size_t)C);
+    const size_t i_res = off; off += con_align(sizeof(cvb_recon_result));
+    const size_t i_pout = off; off += con_align(sizeof(cvb_pose) * V);
+    const size_t i_vs = off; off += con_align(V);
+    const size_t i_os = off; off += con_align(no);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->out.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->out.p;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_pose, poses, sizeof(cvb_pose) * V, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_vo, vo, sizeof(uint32_t) * (V + 1), cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_vl, vl, sizeof(uint32_t) * (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_bear, bear, sizeof(double) * 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_lo, lo, sizeof(uint32_t) * ((size_t)L + 1), cudaMemcpyHostToDevice, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_obs, obs, sizeof(uint32_t) * 2 * (size_t)no, cudaMemcpyHostToDevice, st));
+    if (C) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_cons, cons, sizeof(cvb_view_constraint) * (size_t)C, cudaMemcpyHostToDevice, st));
+    if ((rc = optimize_reconstruction_dev(ctx, cfg, tri, V, (const cvb_pose *)(b + i_pose), (const uint32_t *)(b + i_vo),
+                                          (const uint32_t *)(b + i_vl), (const double *)(b + i_bear), nf, L, (const uint32_t *)(b + i_lo),
+                                          (const uint32_t *)(b + i_obs), no, (const cvb_view_constraint *)(b + i_cons), C,
+                                          (cvb_recon_result *)(b + i_res), (cvb_pose *)(b + i_pout), b + i_vs, b + i_os)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, b + i_res, sizeof(cvb_recon_result), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, b + i_pout, sizeof(cvb_pose) * V, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(view_state, b + i_vs, V, cudaMemcpyDeviceToHost, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(obs_state, b + i_os, no, cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
