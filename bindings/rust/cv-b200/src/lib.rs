@@ -213,3 +213,6 @@ pub mod constraints;
 
 // ---- INTEGRATION.md section 2n (include/cvb200_reconstruction.h) ----
 pub mod reconstruction;
+
+// ---- INTEGRATION.md section 2o (include/cvb200_export.h) ----
+pub mod export;

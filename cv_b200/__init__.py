@@ -25,6 +25,9 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   optimize_reconstruction, regenerate_reconstruction, ReconstructionSettings <- cv-sfm VSlam::optimize_reconstruction /
                            regenerate_reconstruction (cv-sfm/src/lib.rs:2343-2435): the three-view pose graph and the observation
                            filter of one reconstruction snapshot in one call
+  robust_landmarks, normalize_reconstruction, export_reconstruction, ExportSettings <- cv-sfm VSlam::triangulate_landmark_robust /
+                           normalize_reconstruction / export_reconstruction (cv-sfm/src/lib.rs:2241-2340, 2907-3000) of one
+                           reconstruction snapshot in one call each
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -54,5 +57,6 @@ from .pair import (InitSettings, Intrinsics, IntrinsicsK1, TwoViewBuffers, init_
 from .features import frame_features  # noqa: F401
 from .constraints import ConstraintSettings, generate_view_constraints  # noqa: F401
 from .reconstruction import ReconstructionSettings, optimize_reconstruction, regenerate_reconstruction  # noqa: F401
+from .export import ExportSettings, export_reconstruction, normalize_reconstruction, robust_landmarks  # noqa: F401
 
 __version__ = "0.1.0"

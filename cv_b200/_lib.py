@@ -3,7 +3,7 @@ cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (i
 (include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
 (include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h) and cv_b200/libcvb200_reconstruction.so
-(include/cvb200_reconstruction.h)."""
+(include/cvb200_reconstruction.h) and cv_b200/libcvb200_export.so (include/cvb200_export.h)."""
 import ctypes as C
 import os
 
@@ -132,6 +132,12 @@ CONSTRAINTS_MAX_LANDMARKS = 512
 # checked by tests/test_abi_reconstruction.py
 RECONSTRUCTION_ABI_SYMBOLS = ["cvb_recon_cfg_default", "cvb_optimize_reconstruction_check", "cvb_optimize_reconstruction_dev",
                               "cvb_optimize_reconstruction"]
+
+# every symbol include/cvb200_export.h declares (cv-sfm's reconstruction export), exported by libcvb200_export.so; checked by
+# tests/test_abi_export.py
+EXPORT_ABI_SYMBOLS = ["cvb_export_cfg_default", "cvb_export_check", "cvb_robust_landmarks_dev", "cvb_robust_landmarks",
+                      "cvb_export_reconstruction_dev", "cvb_export_reconstruction", "cvb_normalize_reconstruction_dev",
+                      "cvb_normalize_reconstruction"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -416,6 +422,36 @@ def load_reconstruction_library():
         L.cvb_optimize_reconstruction.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u32, vp, vp, vp, vp]
         _RECONSTRUCTION_LIB = L
     return _RECONSTRUCTION_LIB
+
+
+_EXPORT_LIB = None
+
+
+def export_lib_path():
+    return os.path.join(_HERE, "libcvb200_export.so")
+
+
+def load_export_library():
+    """Loads libcvb200_export.so, the module of include/cvb200_export.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _EXPORT_LIB
+    if _EXPORT_LIB is None:
+        load_library()
+        p = export_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_export_cfg_default.argtypes = [vp]
+        L.cvb_export_cfg_default.restype = None
+        L.cvb_export_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32, u32]
+        L.cvb_robust_landmarks_dev.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, vp]
+        L.cvb_robust_landmarks.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, vp]
+        L.cvb_export_reconstruction_dev.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, vp, vp, vp, vp]
+        L.cvb_export_reconstruction.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, vp, vp]
+        L.cvb_normalize_reconstruction_dev.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, u32, u32, vp, vp, vp]
+        L.cvb_normalize_reconstruction.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u32, u32, vp, vp, vp]
+        _EXPORT_LIB = L
+    return _EXPORT_LIB
 
 
 class Context:

@@ -78,7 +78,15 @@ __global__ void __launch_bounds__(256) k_con_gather_obs(const cvb_pose *__restri
     for (int r = 0; r < 3; r++) obs_bear[3 * (size_t)o + r] = b[r];
     world_bearing(P, b, obs_world + 3 * (size_t)o);
 }
-// triangulate_landmark_robust is Some (lib.rs:2907-2934, 2975-3000); one thread per landmark
+// triangulate_landmark_robust (lib.rs:2907-2934, 2975-3000) of the landmark whose n gathered observations start at o0: 0 when its
+// observations are not robust, 1 when the triangulator returns None, 2 when it returns the point p
+__device__ __forceinline__ int robust_landmark_point(const cvb_triangulator &T, uint32_t o0, uint32_t n, const cvb_pose *obs_pose,
+                                                     const double *obs_bear, const double *obs_world, double *W, uint32_t min_obs,
+                                                     double inc, double *p) {
+    if (!observations_robust(obs_world, o0, n, min_obs, inc)) return 0;
+    return triangulate_observations(T, obs_pose + o0, obs_bear + 3 * (size_t)o0, n, W ? W + 6 * (size_t)o0 : nullptr, p) ? 2 : 1;
+}
+// triangulate_landmark_robust is Some; one thread per landmark
 __global__ void __launch_bounds__(128) k_con_robust(cvb_triangulator T, const uint32_t *__restrict__ lm_off, uint32_t L,
                                                     const cvb_pose *__restrict__ obs_pose, const double *__restrict__ obs_bear,
                                                     const double *__restrict__ obs_world, double *__restrict__ W, ConParams prm,
@@ -86,12 +94,8 @@ __global__ void __launch_bounds__(128) k_con_robust(cvb_triangulator T, const ui
     const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= L) return;
     const uint32_t o0 = lm_off[l], n = lm_off[l + 1] - o0;
-    bool ok = observations_robust(obs_world, o0, n, prm.min_obs, prm.inc);
-    if (ok) {
-        double p[4];
-        ok = triangulate_observations(T, obs_pose + o0, obs_bear + 3 * (size_t)o0, n, W ? W + 6 * (size_t)o0 : nullptr, p);
-    }
-    robust[l] = ok ? 1 : 0;
+    double p[4];
+    robust[l] = robust_landmark_point(T, o0, n, obs_pose, obs_bear, obs_world, W, prm.min_obs, prm.inc, p) == 2 ? 1 : 0;
 }
 // view_covisibilities (lib.rs:2535-2556): the query's robust landmarks in feature order, the landmarks per other view, and the coviews
 // kept (lib.rs:2443-2450), ascending; cnt (Qc x V, zeroed) counts, kidx (Qc x V) is the kept position or CON_NONE, kview the kept views

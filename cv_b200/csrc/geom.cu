@@ -22,6 +22,7 @@
 #include "../../include/cvb200_init.h"
 #include "../../include/cvb200_constraints.h"
 #include "../../include/cvb200_reconstruction.h"
+#include "../../include/cvb200_export.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1575,6 +1576,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 #include "init_dev.cuh"
 #include "constraints_dev.cuh"
 #include "reconstruction_dev.cuh"
+#include "export_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1735,12 +1737,13 @@ struct GeomWorkspace {
     DevBuf init;                    // the three-view initialisation's per-call workspace (init_reconstruction_dev)
     DevBuf con, con2;               // the view constraints' snapshot / per-chunk and per-sub-chunk workspaces (view_constraints_dev)
     DevBuf rec;                     // the reconstruction optimisation's workspace (optimize_reconstruction_dev)
+    DevBuf exp;                     // the export's workspace (export_dev.cuh's drivers)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2, &g->rec};
+                      &g->con2, &g->rec, &g->exp};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -3327,6 +3330,301 @@ int optimize_reconstruction(cvb_ctx *ctx, const cvb_recon_cfg *cfg, const cvb_tr
     CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, b + i_pout, sizeof(cvb_pose) * V, cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cudaMemcpyAsync(view_state, b + i_vs, V, cudaMemcpyDeviceToHost, st));
     if (no) CVB_CUDA(ctx, cudaMemcpyAsync(obs_state, b + i_os, no, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+// ---- cv-sfm's reconstruction export (C names in export_abi.cu, include/cvb200_export.h; kernels in export_dev.cuh) --------------------
+void export_cfg_default(cvb_export_cfg *c) {
+    if (!c) return;
+    memset(c, 0, sizeof(*c));
+    c->robust_observation_incidence_minimum_cosine_distance = 1e-3;
+    c->robust_minimum_observations = 3;
+}
+
+int export_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                 const cvb_view_constraint *cons, uint32_t C, uint32_t first_view) {
+    if (optimize_reconstruction_check(V, vo, vl, L, lo, obs, cons, C)) return CVB_EINVAL;
+    return first_view < V ? 0 : CVB_EINVAL;
+}
+
+namespace {
+
+// the arguments every export entry checks; n_features against view_offsets[V] (read back)
+int export_args(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const uint32_t *view_off_dev,
+                uint32_t n_features) {
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: the export takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    uint32_t nf = 0;
+    CVB_CUDA(ctx, cudaMemcpyAsync(&nf, view_off_dev + V, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    if (nf != n_features) return cvb_set_error(ctx, CVB_EINVAL, "view_offsets[V] = %u, n_features %u", nf, n_features);
+    return 0;
+}
+
+// the robust points and states of every landmark (list == nullptr) or of the n landmarks in list, into the workspace; block_cnt (may be
+// nullptr) gets the POINT count of every CTA of EXP_NT landmarks
+struct ExpRobust { double *points; uint8_t *state; uint32_t *block_cnt, *n_points; };
+int export_robust(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                  const uint32_t *view_off_dev, const double *bear_dev, uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev,
+                  uint32_t n_obs, const uint32_t *list, uint32_t n, bool count, ExpRobust &out) {
+    const uint32_t nb = cdiv(std::max<uint32_t>(L, 1), EXP_NT);
+    size_t off = 0;
+    const size_t o_pose = off; off += con_align(sizeof(cvb_pose) * std::max<size_t>(n_obs, 1));
+    const size_t o_bear = off; off += con_align(sizeof(double) * 3 * std::max<size_t>(n_obs, 1));
+    const size_t o_world = off; off += con_align(sizeof(double) * 3 * std::max<size_t>(n_obs, 1));
+    const size_t o_W = off; off += tri->method == CVB_TRI_SINE_L1 ? con_align(sizeof(double) * 6 * std::max<size_t>(n_obs, 1)) : 0;
+    const size_t o_pts = off; off += con_align(sizeof(double) * 4 * std::max<size_t>(L, 1));
+    const size_t o_state = off; off += con_align(std::max<size_t>(L, 1));
+    const size_t o_cnt = off; off += con_align(sizeof(uint32_t) * ((size_t)nb + 1));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->exp.ensure(ctx, off))) return rc;
+    unsigned char *base = (unsigned char *)g->exp.p;
+    cvb_pose *obs_pose = (cvb_pose *)(base + o_pose);
+    double *obs_bear = (double *)(base + o_bear), *obs_world = (double *)(base + o_world);
+    double *W = tri->method == CVB_TRI_SINE_L1 ? (double *)(base + o_W) : nullptr;
+    out.points = (double *)(base + o_pts);
+    out.state = base + o_state;
+    out.block_cnt = (uint32_t *)(base + o_cnt);
+    out.n_points = out.block_cnt + nb;
+    cudaStream_t st = ctx->stream;
+    if (n_obs) {
+        CVB_PROF(ctx, "k_con_gather_obs", 0);
+        k_con_gather_obs<<<cdiv(n_obs, 256), 256, 0, st>>>(poses_dev, view_off_dev, bear_dev, obs_dev, n_obs, obs_pose, obs_bear, obs_world);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (n) {
+        CVB_PROF(ctx, "k_exp_robust", 0);
+        k_exp_robust<<<cdiv(n, EXP_NT), EXP_NT, 0, st>>>(*tri, lm_off_dev, list, n, obs_pose, obs_bear, obs_world, W,
+                                                         std::min(cfg->robust_minimum_observations, V),
+                                                         cfg->robust_observation_incidence_minimum_cosine_distance, out.points, out.state,
+                                                         count ? out.block_cnt : nullptr);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return 0;
+}
+
+}  // namespace
+
+int robust_landmarks_dev(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                         const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, uint32_t n_features, uint32_t L,
+                         const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs, double *points_dev, uint8_t *state_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses_dev || !view_off_dev || !lm_off_dev || (n_features && (!view_lm_dev || !bear_dev)) || (n_obs && !obs_dev) ||
+        (L && (!points_dev || !state_dev)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    int rc;
+    if ((rc = export_args(ctx, cfg, tri, V, view_off_dev, n_features))) return rc;
+    ExpRobust r;
+    if ((rc = export_robust(ctx, cfg, tri, V, poses_dev, view_off_dev, bear_dev, L, lm_off_dev, obs_dev, n_obs, nullptr, L, false, r))) return rc;
+    cudaStream_t st = ctx->stream;
+    if (L) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(points_dev, r.points, sizeof(double) * 4 * (size_t)L, cudaMemcpyDeviceToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(state_dev, r.state, L, cudaMemcpyDeviceToDevice, st));
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int export_reconstruction_dev(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                              const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, const uint8_t *colors_dev,
+                              uint32_t n_features, uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs,
+                              double *points_dev, uint8_t *colors_out_dev, uint32_t *n_points_dev, cvb_export_camera *cameras_dev,
+                              double *mean_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses_dev || !view_off_dev || !lm_off_dev || !n_points_dev || !cameras_dev ||
+        (n_features && (!view_lm_dev || !bear_dev || !colors_dev)) || (n_obs && !obs_dev) || (L && (!points_dev || !colors_out_dev)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    int rc;
+    if ((rc = export_args(ctx, cfg, tri, V, view_off_dev, n_features))) return rc;
+    ExpRobust r;
+    if ((rc = export_robust(ctx, cfg, tri, V, poses_dev, view_off_dev, bear_dev, L, lm_off_dev, obs_dev, n_obs, nullptr, L, true, r))) return rc;
+    cudaStream_t st = ctx->stream;
+    const uint32_t nb = cdiv(L, EXP_NT);
+    {
+        CVB_PROF(ctx, "k_exp_compact", 0);
+        k_exp_scan<<<1, 32, 0, st>>>(nb, r.block_cnt, r.n_points);
+        CVB_LAUNCH_CHECK(ctx);
+        if (L) {
+            k_exp_compact<<<nb, EXP_NT, 0, st>>>(L, r.points, r.state, r.block_cnt, view_off_dev, lm_off_dev, obs_dev, colors_dev, points_dev,
+                                                 colors_out_dev);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        CVB_CUDA(ctx, cudaMemcpyAsync(n_points_dev, r.n_points, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    }
+    {
+        CVB_PROF(ctx, "k_exp_cameras", 0);
+        k_exp_cameras<<<cdiv((size_t)V * 32, 256), 256, 0, st>>>(V, poses_dev, view_off_dev, view_lm_dev, r.points, r.state, cameras_dev,
+                                                                 mean_dev);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int normalize_reconstruction_dev(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses_dev,
+                                 const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, uint32_t n_features,
+                                 uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs,
+                                 const cvb_view_constraint *cons_dev, uint32_t C, uint32_t first_view, cvb_pose *poses_out_dev,
+                                 cvb_view_constraint *cons_out_dev, cvb_normalize_result *res_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses_dev || !view_off_dev || !lm_off_dev || !poses_out_dev || !res_dev ||
+        (n_features && (!view_lm_dev || !bear_dev)) || (n_obs && !obs_dev) || (C && (!cons_dev || !cons_out_dev)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (V && first_view >= V) return cvb_set_error(ctx, CVB_EINVAL, "first_view %u of %u views", first_view, V);
+    int rc;
+    if ((rc = export_args(ctx, cfg, tri, V, view_off_dev, n_features))) return rc;
+    cudaStream_t st = ctx->stream;
+    // only the first view's landmarks are triangulated: their list is the view's stretch of view_landmarks
+    uint32_t f[2];
+    CVB_CUDA(ctx, cudaMemcpyAsync(f, view_off_dev + first_view, sizeof(f), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    ExpRobust r;
+    if ((rc = export_robust(ctx, cfg, tri, V, poses_dev, view_off_dev, bear_dev, L, lm_off_dev, obs_dev, n_obs, view_lm_dev + f[0], f[1] - f[0],
+                            false, r)))
+        return rc;
+    {
+        CVB_PROF(ctx, "k_exp_normalize", 0);
+        k_exp_first_mean<<<1, 32, 0, st>>>(first_view, poses_dev, view_off_dev, view_lm_dev, r.points, r.state, res_dev);
+        CVB_LAUNCH_CHECK(ctx);
+        k_exp_normalize<<<cdiv(std::max(V, C), 256), 256, 0, st>>>(V, C, first_view, poses_dev, cons_dev, res_dev, poses_out_dev, cons_out_dev);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+namespace {
+
+// the snapshot's host arrays into the context's output workspace; the offsets of what follows them start at `off`
+struct ExpUpload { size_t pose, vo, vl, bear, col, lo, obs, cons, end; };
+int export_upload(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear,
+                  const uint8_t *colors, uint32_t L, const uint32_t *lo, const uint32_t *obs, const cvb_view_constraint *cons, uint32_t C,
+                  size_t extra, ExpUpload &u, unsigned char *&b) {
+    const uint32_t nf = vo[V], no = lo[L];
+    size_t off = 0;
+    u.pose = off; off += con_align(sizeof(cvb_pose) * V);
+    u.vo = off; off += con_align(sizeof(uint32_t) * (V + 1));
+    u.vl = off; off += con_align(sizeof(uint32_t) * (size_t)nf);
+    u.bear = off; off += con_align(sizeof(double) * 3 * (size_t)nf);
+    u.col = off; off += con_align(3 * (size_t)nf);
+    u.lo = off; off += con_align(sizeof(uint32_t) * ((size_t)L + 1));
+    u.obs = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)no);
+    u.cons = off; off += con_align(sizeof(cvb_view_constraint) * (size_t)C);
+    u.end = off;
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = g->out.ensure(ctx, off + extra))) return rc;
+    b = (unsigned char *)g->out.p;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + u.pose, poses, sizeof(cvb_pose) * V, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + u.vo, vo, sizeof(uint32_t) * (V + 1), cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + u.vl, vl, sizeof(uint32_t) * (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(b + u.bear, bear, sizeof(double) * 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (nf && colors) CVB_CUDA(ctx, cudaMemcpyAsync(b + u.col, colors, 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + u.lo, lo, sizeof(uint32_t) * ((size_t)L + 1), cudaMemcpyHostToDevice, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(b + u.obs, obs, sizeof(uint32_t) * 2 * (size_t)no, cudaMemcpyHostToDevice, st));
+    if (C) CVB_CUDA(ctx, cudaMemcpyAsync(b + u.cons, cons, sizeof(cvb_view_constraint) * (size_t)C, cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+}  // namespace
+
+int robust_landmarks(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                     const uint32_t *vo, const uint32_t *vl, const double *bear, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                     double *points, uint8_t *state) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (export_check(V, vo, vl, L, lo, obs, nullptr, 0, 0)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot");
+    if ((vo[V] && !bear) || (L && (!points || !state))) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    ExpUpload u;
+    unsigned char *b;
+    const size_t i_pts = con_align(sizeof(double) * 4 * (size_t)L);
+    int rc;
+    if ((rc = export_upload(ctx, V, poses, vo, vl, bear, nullptr, L, lo, obs, nullptr, 0, i_pts + con_align(L), u, b))) return rc;
+    double *pts = (double *)(b + u.end);
+    uint8_t *stt = b + u.end + i_pts;
+    if ((rc = robust_landmarks_dev(ctx, cfg, tri, V, (const cvb_pose *)(b + u.pose), (const uint32_t *)(b + u.vo), (const uint32_t *)(b + u.vl),
+                                   (const double *)(b + u.bear), vo[V], L, (const uint32_t *)(b + u.lo), (const uint32_t *)(b + u.obs), lo[L],
+                                   pts, stt)))
+        return rc;
+    cudaStream_t st = ctx->stream;
+    if (L) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(points, pts, sizeof(double) * 4 * (size_t)L, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(state, stt, L, cudaMemcpyDeviceToHost, st));
+    }
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int export_reconstruction(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                          const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *colors, uint32_t L, const uint32_t *lo,
+                          const uint32_t *obs, double *points, uint8_t *point_colors, uint32_t *n_points, cvb_export_camera *cameras,
+                          double *mean) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses || !n_points || !cameras) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (export_check(V, vo, vl, L, lo, obs, nullptr, 0, 0)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot");
+    if ((vo[V] && (!bear || !colors)) || (L && (!points || !point_colors))) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    size_t x = 0;
+    const size_t i_pts = x; x += con_align(sizeof(double) * 3 * (size_t)L);
+    const size_t i_col = x; x += con_align(3 * (size_t)L);
+    const size_t i_n = x; x += con_align(sizeof(uint32_t));
+    const size_t i_cam = x; x += con_align(sizeof(cvb_export_camera) * V);
+    const size_t i_mean = x; x += con_align(sizeof(double) * V);
+    ExpUpload u;
+    unsigned char *b;
+    int rc;
+    if ((rc = export_upload(ctx, V, poses, vo, vl, bear, colors, L, lo, obs, nullptr, 0, x, u, b))) return rc;
+    unsigned char *o = b + u.end;
+    if ((rc = export_reconstruction_dev(ctx, cfg, tri, V, (const cvb_pose *)(b + u.pose), (const uint32_t *)(b + u.vo),
+                                        (const uint32_t *)(b + u.vl), (const double *)(b + u.bear), b + u.col, vo[V], L,
+                                        (const uint32_t *)(b + u.lo), (const uint32_t *)(b + u.obs), lo[L], (double *)(o + i_pts), o + i_col,
+                                        (uint32_t *)(o + i_n), (cvb_export_camera *)(o + i_cam), (double *)(o + i_mean))))
+        return rc;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(n_points, o + i_n, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(cameras, o + i_cam, sizeof(cvb_export_camera) * V, cudaMemcpyDeviceToHost, st));
+    if (mean) CVB_CUDA(ctx, cudaMemcpyAsync(mean, o + i_mean, sizeof(double) * V, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (*n_points) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(points, o + i_pts, sizeof(double) * 3 * (size_t)*n_points, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(point_colors, o + i_col, 3 * (size_t)*n_points, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+    }
+    return 0;
+}
+
+int normalize_reconstruction(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                             const uint32_t *vo, const uint32_t *vl, const double *bear, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                             const cvb_view_constraint *cons, uint32_t C, uint32_t first_view, cvb_pose *poses_out,
+                             cvb_view_constraint *cons_out, cvb_normalize_result *res) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !poses || !poses_out || !res || (C && !cons_out)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (export_check(V, vo, vl, L, lo, obs, cons, C, first_view)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot or constraints");
+    if (vo[V] && !bear) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    size_t x = 0;
+    const size_t i_pout = x; x += con_align(sizeof(cvb_pose) * V);
+    const size_t i_cout = x; x += con_align(sizeof(cvb_view_constraint) * (size_t)C);
+    const size_t i_res = x; x += con_align(sizeof(cvb_normalize_result));
+    ExpUpload u;
+    unsigned char *b;
+    int rc;
+    if ((rc = export_upload(ctx, V, poses, vo, vl, bear, nullptr, L, lo, obs, cons, C, x, u, b))) return rc;
+    unsigned char *o = b + u.end;
+    if ((rc = normalize_reconstruction_dev(ctx, cfg, tri, V, (const cvb_pose *)(b + u.pose), (const uint32_t *)(b + u.vo),
+                                           (const uint32_t *)(b + u.vl), (const double *)(b + u.bear), vo[V], L, (const uint32_t *)(b + u.lo),
+                                           (const uint32_t *)(b + u.obs), lo[L], (const cvb_view_constraint *)(b + u.cons), C, first_view,
+                                           (cvb_pose *)(o + i_pout), (cvb_view_constraint *)(o + i_cout), (cvb_normalize_result *)(o + i_res))))
+        return rc;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, o + i_pout, sizeof(cvb_pose) * V, cudaMemcpyDeviceToHost, st));
+    if (C) CVB_CUDA(ctx, cudaMemcpyAsync(cons_out, o + i_cout, sizeof(cvb_view_constraint) * (size_t)C, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, o + i_res, sizeof(cvb_normalize_result), cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
