@@ -131,7 +131,7 @@ struct AkazeWorkspace {
     unsigned *rowcount = nullptr, *rowoff = nullptr, *ncand = nullptr;
     Cand *cand = nullptr;
     cvb_keypoint *cache = nullptr, *refined = nullptr, *sorted = nullptr;
-    unsigned *ncache = nullptr, *nsorted = nullptr, *nvalid = nullptr, *rank = nullptr;
+    unsigned *ncache = nullptr, *nneed = nullptr, *nsorted = nullptr, *nvalid = nullptr, *rank = nullptr;   // nneed: unclamped cache count
     unsigned char *keep = nullptr, *valid = nullptr, *ok = nullptr, *desc_tmp = nullptr;
     unsigned *overflow = nullptr;
     CUtensorMap *tmaps = nullptr;      // device: [3][MAX_EVO] per-evolution maps (deriv1 source, Lx, Ly) for the TMA-staged tiles
@@ -154,6 +154,7 @@ struct AkazeWorkspace {
     unsigned *n_out = nullptr;
     unsigned cap_out = 0;
     std::vector<void *> allocs;
+    std::vector<void *> kp_allocs;   // the buffers sized by capc / capk, replaced when a frame needs more (grow_keypoint_capacity)
     bool has_run = false;
     // second stream for the detector response of finished octaves (overlaps the latency-bound coarse octaves)
     cudaStream_t aux = nullptr;
@@ -184,6 +185,7 @@ void akaze_workspace_free(AkazeWorkspace *ws) {
     for (cudaEvent_t e : ws->ev_fork) if (e) cudaEventDestroy(e);
     if (ws->ev_join) cudaEventDestroy(ws->ev_join);
     for (void *p : ws->allocs) cudaFree(p);
+    for (void *p : ws->kp_allocs) cudaFree(p);
     for (void *p : {(void *)ws->st_kp, (void *)ws->st_kp_out, (void *)ws->st_ok, (void *)ws->st_desc, (void *)ws->st_desc_out,
                     (void *)ws->st_off, (void *)ws->st_n, (void *)ws->st_need})
         if (p) cudaFree(p);
@@ -233,12 +235,59 @@ int fed_fuse_steps() {
 }
 
 template <typename T>
-int dalloc(cvb_ctx *ctx, AkazeWorkspace *ws, T **p, size_t n) {
+int dalloc_into(cvb_ctx *ctx, std::vector<void *> &list, T **p, size_t n) {
     void *q = nullptr;
     cudaError_t e = cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T));
     if (e != cudaSuccess) return cvb_set_error(ctx, CVB_ENOMEM, "cudaMalloc(%zu bytes): %s", n * sizeof(T), cudaGetErrorString(e));
-    ws->allocs.push_back(q);
+    list.push_back(q);
     *p = (T *)q;
+    return 0;
+}
+
+template <typename T>
+int dalloc(cvb_ctx *ctx, AkazeWorkspace *ws, T **p, size_t n) { return dalloc_into(ctx, ws->allocs, p, n); }
+
+// the buffers of the keypoint stages sized by the workspace's capacities: capc candidates, capk cached keypoints (per frame)
+int alloc_keypoint_buffers(cvb_ctx *ctx, AkazeWorkspace *ws) {
+    const size_t B = ws->batch;
+    int rc = 0;
+#define DK(p, n) do { rc = dalloc_into(ctx, ws->kp_allocs, &ws->p, (n)); if (rc) return rc; } while (0)
+    DK(cand, B * ws->capc);
+    DK(sup.state, B * ws->capc); DK(sup.alive, B * ws->capc); DK(sup.rdy, B * ws->capc);
+    DK(sup.key, B * ws->capc); DK(sup.rank, B * ws->capc); DK(sup.next, B * ws->capc);
+    DK(cache, B * ws->capk); DK(refined, B * ws->capk); DK(sorted, B * ws->capk); DK(rank, B * ws->capk);
+    DK(keep, B * ws->capk); DK(valid, B * ws->capk); DK(ok, B * ws->capk); DK(desc_tmp, B * ws->capk * 64);
+#undef DK
+    return 0;
+}
+
+// Grow the capacities to at least (need_c, need_k), keeping every plane (and so a staged scale space and its ticket).  The
+// captured graphs hold the old buffers and are dropped.  The keypoint-stage buffers hold nothing between calls.  The new set is
+// allocated before the old one is freed: when an allocation fails, the workspace keeps its buffers and capacities and stays usable.
+int grow_keypoint_capacity(cvb_ctx *ctx, AkazeWorkspace *ws, size_t need_c, size_t need_k) {
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    for (auto &g : ws->graphs) cudaGraphExecDestroy(g.exec);
+    ws->graphs.clear();
+    AkazeWorkspace *nw = new AkazeWorkspace();
+    nw->batch = ws->batch;
+    // an eighth more than the count, so that a run of similar frames does not grow again at every frame
+    nw->capc = need_c > ws->capc ? (unsigned)std::min<size_t>(need_c + need_c / 8, 0xffffffffu) : ws->capc;
+    nw->capk = need_k > ws->capk ? (unsigned)std::min<size_t>(need_k + need_k / 8, 0xffffffffu) : ws->capk;
+    const int rc = alloc_keypoint_buffers(ctx, nw);
+    if (rc) {
+        for (void *p : nw->kp_allocs) cudaFree(p);
+        delete nw;
+        return rc;
+    }
+    for (void *p : ws->kp_allocs) cudaFree(p);
+    ws->kp_allocs = std::move(nw->kp_allocs);
+    ws->capc = nw->capc; ws->capk = nw->capk;
+    ws->cand = nw->cand;
+    ws->sup.state = nw->sup.state; ws->sup.alive = nw->sup.alive; ws->sup.rdy = nw->sup.rdy;
+    ws->sup.key = nw->sup.key; ws->sup.rank = nw->sup.rank; ws->sup.next = nw->sup.next;
+    ws->cache = nw->cache; ws->refined = nw->refined; ws->sorted = nw->sorted; ws->rank = nw->rank;
+    ws->keep = nw->keep; ws->valid = nw->valid; ws->ok = nw->ok; ws->desc_tmp = nw->desc_tmp;
+    delete nw;   // its buffers now belong to ws
     return 0;
 }
 
@@ -426,7 +475,9 @@ int build_workspace(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, 
     if (make_gauss_taps((float)cfg->base_scale_offset, &ws->g0)) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "base_scale_offset too large");
     make_gauss_taps(1.0f, &ws->g1);
     ws->p0 = (size_t)w * h;
-    // capacities: every strict 3x3 maximum needs a 2-pixel pitch -> at most P/4 per level; bound generously
+    // capacities for the frames of everyday threshold and texture: a frame that exceeds them makes the host calls grow them
+    // (grow_keypoint_capacity) and run again; the _dev calls report it with flag 1 or 2 of cvb_akaze_dev_overflow.  A proven bound
+    // (every strict 3x3 maximum needs a 2-pixel pitch: P/4 per level) would cost ~155 bytes per possible cached keypoint.
     ws->capc = (unsigned)std::min<size_t>(std::max<size_t>(ws->p0 / 8, 4096), 1u << 20);
     ws->capk = (unsigned)std::min<size_t>(std::max<size_t>(ws->p0 / 32, 4096), 1u << 17);
     const size_t B = batch, PF = ws->plane_floats, R = (size_t)std::max(ws->table.total_rows, 1);
@@ -438,11 +489,9 @@ int build_workspace(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, 
     DA(gmax, B); DA(hist, B * cfg->contrast_factor_num_bins); DA(npoints, B); DA(kc, B); DA(inv_k, B * MAX_EVO);
     DA(evo_octave, MAX_EVO);
     DA(rowcount, B * R); DA(rowoff, B * R); DA(ncand, B);
-    DA(cand, B * ws->capc);
-    DA(cache, B * ws->capk); DA(refined, B * ws->capk); DA(sorted, B * ws->capk);
-    DA(ncache, B); DA(nsorted, B); DA(nvalid, B); DA(rank, B * ws->capk);
-    DA(keep, B * ws->capk); DA(valid, B * ws->capk); DA(ok, B * ws->capk); DA(desc_tmp, B * ws->capk * 64);
+    DA(ncache, B); DA(nneed, B); DA(nsorted, B); DA(nvalid, B);
     DA(overflow, 1);
+    if ((rc = alloc_keypoint_buffers(ctx, ws))) return rc;
     {   // scratch of the parallel duplicate suppression; bins sized for the finest class grid
         unsigned nbmax = 1;
         for (size_t i = 0; i < ws->evo.size(); i++) {
@@ -452,8 +501,6 @@ int build_workspace(cvb_ctx *ctx, AkazeWorkspace *ws, const cvb_akaze_cfg *cfg, 
             nbmax = std::max(nbmax, nbx * nby);
         }
         ws->sup.nbmax = nbmax;
-        DA(sup.state, B * ws->capc); DA(sup.alive, B * ws->capc); DA(sup.rdy, B * ws->capc);
-        DA(sup.key, B * ws->capc); DA(sup.rank, B * ws->capc); DA(sup.next, B * ws->capc);
         DA(sup.binA, B * nbmax); DA(sup.binB, B * nbmax);
         const char *env = getenv("CVB_SUPPRESS_SEQ");
         ws->suppress_seq = env && env[0] == '1';
@@ -774,13 +821,14 @@ int stage_detect(cvb_ctx *ctx, unsigned B) {
     }
     { CVB_PROF(ctx, "k_suppress", 0);
     if (ws->suppress_seq)
-        k_suppress_seq<<<B, 1024, 0, st>>>(ws->cand, ws->ncand, ws->capc, ws->table, ws->cache, ws->ncache, ws->capk, ws->overflow);
+        k_suppress_seq<<<B, 1024, 0, st>>>(ws->cand, ws->ncand, ws->capc, ws->table, ws->cache, ws->ncache, ws->nneed, ws->capk,
+                                           ws->overflow);
     else {
         k_suppress_smem<<<B, 1024, SUP_SMEM, st>>>(ws->cand, ws->ncand, ws->rowoff, ws->capc, ws->table, ws->sup, ws->cache,
-                                                   ws->ncache, ws->capk, ws->overflow, ws->sup_fallback);
+                                                   ws->ncache, ws->nneed, ws->capk, ws->overflow, ws->sup_fallback);
         CVB_LAUNCH_CHECK(ctx);
         k_suppress_par<<<B, 1024, 0, st>>>(ws->cand, ws->ncand, ws->rowoff, ws->capc, ws->table, ws->sup, ws->cache, ws->ncache,
-                                           ws->capk, ws->overflow, ws->suppress_par_only ? nullptr : ws->sup_fallback);
+                                           ws->nneed, ws->capk, ws->overflow, ws->suppress_par_only ? nullptr : ws->sup_fallback);
     }
     CVB_LAUNCH_CHECK(ctx); }
     const unsigned kp_blocks = (unsigned)ctx->num_sms * 2;
@@ -892,6 +940,7 @@ int check_args(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const void *img, uint32_t
     return 0;
 }
 
+
 }  // namespace
 
 extern "C" {
@@ -938,6 +987,39 @@ int cvb_akaze_extract_batch(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float 
 
 }  // extern "C"
 
+// Clears the overflow flag on the context's stream, so that the flag a host call reads back belongs to that call alone.
+int akaze_clear_overflow(cvb_ctx *ctx) {
+    if (ctx->akaze) CVB_CUDA(ctx, cudaMemsetAsync(ctx->akaze->overflow, 0, sizeof(unsigned), ctx->stream));
+    return 0;
+}
+
+// The host calls' answer to an overflow flag of their last detection (B frames): did a frame need more than capc candidates or
+// capk cached keypoints?  ncand is never clamped.  nneed is exact when every candidate fit; when the candidates were clamped at
+// capc the suppression saw only the first capc of them, so nneed can fall short of the frame's need and a second rerun can be
+// needed.  *rerun: the capacities were grown to the need and the detection is to run again.  After MAX_CAPACITY_RERUNS reruns an
+// exceeded capacity is CVB_ECAP.
+int akaze_capacity_rerun(cvb_ctx *ctx, unsigned B, int attempt, bool *rerun) {
+    constexpr int MAX_CAPACITY_RERUNS = 2;
+    AkazeWorkspace *ws = ctx->akaze;
+    cudaStream_t st = ctx->stream;
+    *rerun = false;
+    unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * 2 * (size_t)B);
+    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->ncand, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(hs + B, ws->nneed, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    size_t need_c = 0, need_k = 0;
+    for (unsigned b = 0; b < B; b++) { need_c = std::max<size_t>(need_c, hs[b]); need_k = std::max<size_t>(need_k, hs[B + b]); }
+    if (need_c <= ws->capc && need_k <= ws->capk) return 0;
+    if (attempt >= MAX_CAPACITY_RERUNS)
+        return cvb_set_error(ctx, CVB_ECAP, "internal keypoint capacity exceeded after %d reruns", MAX_CAPACITY_RERUNS);
+    int rc = grow_keypoint_capacity(ctx, ws, need_c, need_k);
+    if (rc) return rc;
+    CVB_CUDA(ctx, cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st));
+    *rerun = true;
+    return 0;
+}
+
 int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, bool images_on_device, uint32_t batch, uint32_t w,
                              uint32_t h, cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out) {
     int rc = check_args(ctx, cfg, images, batch, w, h);
@@ -950,20 +1032,30 @@ int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float
     cudaStream_t st = ctx->stream;
     if (!images_on_device) CVB_CUDA(ctx, cudaMemcpyAsync(ws->img, images, sizeof(float) * ws->p0 * batch, cudaMemcpyHostToDevice, st));
     const unsigned cap_dev = ws->cap_out;
-    rc = run_extract(ctx, images_on_device ? images : ws->img, batch, ws->kp_out, ws->desc_out, cap_dev, ws->n_out);
-    if (rc) return rc;
-    unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * ((size_t)batch + 1));
-    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->n_out, sizeof(unsigned) * batch, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs + batch, ws->overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cvb_wait(ctx, st));
-    const unsigned ovf = hs[batch];
-    for (uint32_t b = 0; b < batch; b++) n_out[b] = hs[b];
-    if (ovf) {
-        cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st);
-        if (ovf == 3) return cvb_set_error(ctx, CVB_ECAP, "output capacity %u too small", cap);
-        return cvb_set_error(ctx, CVB_ECAP, "internal keypoint capacity exceeded (stage %u)", ovf);
+    // the frames stay resident, so a frame that exceeds the keypoint capacities is run again in a grown workspace
+    if ((rc = akaze_clear_overflow(ctx))) return rc;
+    bool out_full = false;
+    for (int attempt = 0;; attempt++) {
+        rc = run_extract(ctx, images_on_device ? images : ws->img, batch, ws->kp_out, ws->desc_out, cap_dev, ws->n_out);
+        if (rc) return rc;
+        unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * ((size_t)batch + 1));
+        if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->n_out, sizeof(unsigned) * batch, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs + batch, ws->overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        const unsigned ovf = hs[batch];
+        for (uint32_t b = 0; b < batch; b++) n_out[b] = hs[b];
+        if (!ovf) break;
+        bool rerun = false;
+        if ((rc = akaze_capacity_rerun(ctx, batch, attempt, &rerun))) return rc;
+        if (rerun) continue;
+        out_full = ovf == 3;
+        CVB_CUDA(ctx, cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st));
+        break;
     }
+    // the workspace's outputs may hold more than `cap` (a workspace built for a larger cap), so the counts decide too
+    for (uint32_t b = 0; b < batch; b++) out_full = out_full || n_out[b] > cap;
+    if (out_full) return cvb_set_error(ctx, CVB_ECAP, "output capacity %u too small", cap);
     for (uint32_t b = 0; b < batch; b++) {
         unsigned n = std::min<unsigned>(n_out[b], cap);
         if (!n) continue;
@@ -1066,36 +1158,45 @@ int stages_find(cvb_ctx *ctx, uint64_t ticket, cvb_keypoint *kp_out, uint32_t ca
         else memset(n_out, 0, sizeof(unsigned) * B);
         return 0;
     }
-    // detection runs on every call, so that every find reports its own capacity overflows (flags 1 and 2).  It reads the planes
-    // and the per-row extrema counts of the scale space; the unfused extrema mask adds to those counts, so they restart from 0.
-    if (!(ws->deriv_v3 && ws->fuse_det))
-        CVB_CUDA(ctx, cudaMemsetAsync(ws->rowcount, 0, sizeof(unsigned) * (size_t)B * ws->table.total_rows, st));
-    if ((rc = stage_detect(ctx, B))) return rc;
-    CompactArgs A{};
-    A.kp_in = ws->refined; A.keep = ws->valid; A.counts = ws->ncache; A.in_stride = ws->capk; A.cap = cap;
-    A.overflow = ws->overflow;
-    if (on_device) {
-        A.kp_out = kp_out; A.n_out = n_out;
-    } else {
-        if ((rc = ws_grow(ctx, &ws->st_kp_out, &ws->st_kp_out_n, (size_t)B * cap))) return rc;
-        if ((rc = ws_grow(ctx, &ws->st_n, &ws->st_n_n, B))) return rc;
-        if ((rc = ws_grow(ctx, &ws->st_need, &ws->st_need_n, B))) return rc;
-        A.kp_out = ws->st_kp_out; A.n_out = ws->st_n; A.need = ws->st_need;
+    // detection runs on every call, so that every _dev find reports its own capacity overflows (flags 1 and 2), and the host call
+    // runs it again in a grown workspace (the planes, and so the ticket, stay).  It reads the planes and the per-row extrema counts
+    // of the scale space; the unfused extrema mask adds to those counts, so they restart from 0.
+    if (!on_device && (rc = akaze_clear_overflow(ctx))) return rc;   // the host call reads back this call's flag alone
+    std::vector<unsigned> got(B), need(B);
+    for (int attempt = 0;; attempt++) {
+        if (!(ws->deriv_v3 && ws->fuse_det))
+            CVB_CUDA(ctx, cudaMemsetAsync(ws->rowcount, 0, sizeof(unsigned) * (size_t)B * ws->table.total_rows, st));
+        if ((rc = stage_detect(ctx, B))) return rc;
+        CompactArgs A{};
+        A.kp_in = ws->refined; A.keep = ws->valid; A.counts = ws->ncache; A.in_stride = ws->capk; A.cap = cap;
+        A.overflow = ws->overflow;
+        if (on_device) {
+            A.kp_out = kp_out; A.n_out = n_out;
+        } else {
+            if ((rc = ws_grow(ctx, &ws->st_kp_out, &ws->st_kp_out_n, (size_t)B * cap))) return rc;
+            if ((rc = ws_grow(ctx, &ws->st_n, &ws->st_n_n, B))) return rc;
+            if ((rc = ws_grow(ctx, &ws->st_need, &ws->st_need_n, B))) return rc;
+            A.kp_out = ws->st_kp_out; A.n_out = ws->st_n; A.need = ws->st_need;
+        }
+        { CVB_PROF(ctx, "k_compact_stage", 0);
+        k_compact_stage<<<B, 1024, 0, st>>>(A);
+        CVB_LAUNCH_CHECK(ctx); }
+        if (on_device) return 0;
+        unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * (2 * (size_t)B + 1));
+        if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->st_n, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs + B, ws->st_need, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs + 2 * B, ws->overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        const unsigned ovf = hs[2 * B];
+        got.assign(hs, hs + B); need.assign(hs + B, hs + 2 * B);
+        if (!ovf) break;
+        bool rerun = false;
+        if ((rc = akaze_capacity_rerun(ctx, B, attempt, &rerun))) return rc;
+        if (rerun) continue;
+        CVB_CUDA(ctx, cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st));
+        break;   // flag 3: the output, handled below
     }
-    { CVB_PROF(ctx, "k_compact_stage", 0);
-    k_compact_stage<<<B, 1024, 0, st>>>(A);
-    CVB_LAUNCH_CHECK(ctx); }
-    if (on_device) return 0;
-    unsigned *hs = (unsigned *)cvb_pinned(ctx, sizeof(unsigned) * (2 * (size_t)B + 1));
-    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs, ws->st_n, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs + B, ws->st_need, sizeof(unsigned) * B, cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs + 2 * B, ws->overflow, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    CVB_CUDA(ctx, cvb_wait(ctx, st));
-    const unsigned ovf = hs[2 * B];
-    std::vector<unsigned> got(hs, hs + B), need(hs + B, hs + 2 * B);
-    if (ovf) CVB_CUDA(ctx, cudaMemsetAsync(ws->overflow, 0, sizeof(unsigned), st));
-    if (ovf == 1 || ovf == 2) return cvb_set_error(ctx, CVB_ECAP, "internal keypoint capacity exceeded (stage %u)", ovf);
     for (unsigned b = 0; b < B; b++)
         if (need[b] > cap) {
             for (unsigned c = 0; c < B; c++) n_out[c] = need[c];

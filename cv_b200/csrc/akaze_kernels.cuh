@@ -1087,15 +1087,16 @@ __global__ void __launch_bounds__(1024) k_scan_rows(const unsigned *__restrict__
 // the cache (:95-116) and are skipped up front.
 __global__ void __launch_bounds__(1024) k_suppress_seq(const Cand *__restrict__ cand, const unsigned *__restrict__ ncand,
                                                    unsigned capc, EvoTable T, cvb_keypoint *__restrict__ cache,
-                                                   unsigned *__restrict__ ncache, unsigned capk, unsigned *overflow) {
+                                                   unsigned *__restrict__ ncache, unsigned *__restrict__ nneed, unsigned capk,
+                                                   unsigned *overflow) {
     __shared__ unsigned s_min[32];
-    __shared__ unsigned s_n;
+    __shared__ unsigned s_n, s_drop;
     const int b = blockIdx.x;
     const Cand *cd = cand + (size_t)b * capc;
     cvb_keypoint *kc = cache + (size_t)b * capk;
     const unsigned n = min(ncand[b], capc);
     const float smax = 10.0f * sqrtf(2.0f);
-    if (threadIdx.x == 0) s_n = 0;
+    if (threadIdx.x == 0) { s_n = 0; s_drop = 0; }
     __syncthreads();
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     for (unsigned ci = 0; ci < n; ci++) {
@@ -1141,13 +1142,13 @@ __global__ void __launch_bounds__(1024) k_suppress_seq(const Cand *__restrict__ 
                     kp.octave = (uint32_t)ev.octave; kp.class_id = (uint32_t)c.e;
                     if (is_repeated) kc[m] = kp;
                     else if (nc < capk) { kc[nc] = kp; s_n = nc + 1; }
-                    else *overflow = 2u;
+                    else { *overflow = 2u; s_drop++; }
                 }
             }
         }
         __syncthreads();
     }
-    if (threadIdx.x == 0) ncache[b] = s_n;
+    if (threadIdx.x == 0) { ncache[b] = s_n; nneed[b] = s_n + s_drop; }   // an upper bound on the need: a drop can hide a later match
 }
 
 // Parallel, provably sequential-equivalent duplicate suppression (scale_space_extrema.rs:61-117).
@@ -1201,7 +1202,7 @@ __device__ __forceinline__ unsigned block_excl_scan_1024(unsigned v, unsigned *s
 __global__ void __launch_bounds__(1024) k_suppress_par(const Cand *__restrict__ cand, const unsigned *__restrict__ ncand,
                                                        const unsigned *__restrict__ rowoff, unsigned capc, EvoTable T,
                                                        SupScratch S, cvb_keypoint *__restrict__ cache,
-                                                       unsigned *__restrict__ ncache, unsigned capk, unsigned *overflow,
+                                                       unsigned *__restrict__ ncache, unsigned *__restrict__ nneed, unsigned capk, unsigned *overflow,
                                                        const unsigned *__restrict__ fallback) {
     __shared__ unsigned s_warp[33];
     __shared__ int s_more;
@@ -1348,7 +1349,7 @@ __global__ void __launch_bounds__(1024) k_suppress_par(const Cand *__restrict__ 
         kp.octave = (uint32_t)ev.octave; kp.class_id = (uint32_t)c.e;
         cache[(size_t)b * capk + k] = kp;
     }
-    if (threadIdx.x == 0) ncache[b] = min(N, capk);
+    if (threadIdx.x == 0) { ncache[b] = min(N, capk); nneed[b] = N; }
 }
 
 // Shared-memory version of k_suppress_par (same algorithm, same outcomes): all mutable per-candidate state
@@ -1361,7 +1362,7 @@ constexpr size_t SUP_SMEM = SUP_CAPS * (3 + 4 + 2 + 4 + 4 + 2) + SUP_NB * 2 * 4;
 __global__ void __launch_bounds__(1024) k_suppress_smem(const Cand *__restrict__ cand, const unsigned *__restrict__ ncand,
                                                         const unsigned *__restrict__ rowoff, unsigned capc, EvoTable T,
                                                         SupScratch S, cvb_keypoint *__restrict__ cache,
-                                                        unsigned *__restrict__ ncache, unsigned capk, unsigned *overflow,
+                                                        unsigned *__restrict__ ncache, unsigned *__restrict__ nneed, unsigned capk, unsigned *overflow,
                                                         unsigned *__restrict__ fallback) {
     extern __shared__ __align__(16) unsigned char smraw[];
     unsigned *s_key = (unsigned *)smraw;                          // [CAPS]
@@ -1537,7 +1538,7 @@ __global__ void __launch_bounds__(1024) k_suppress_smem(const Cand *__restrict__
         kp.octave = (uint32_t)ev.octave; kp.class_id = (uint32_t)c.e;
         cache[(size_t)b * capk + k] = kp;
     }
-    if (threadIdx.x == 0) ncache[b] = min(N, capk);
+    if (threadIdx.x == 0) { ncache[b] = min(N, capk); nneed[b] = N; }
 }
 
 // Upper-scale filter (:120-140): cache[i] is dropped when a LATER cache entry of class+1 lies within

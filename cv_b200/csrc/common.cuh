@@ -75,6 +75,10 @@ void lsh_workspace_free(LshWorkspace *ws);
 // Bodies of the host-API entry points cvb_akaze_extract_batch, cvb_frame_features_batch and cvb_two_view_frames_k1.  With the
 // *_on_device flag set, the f32 planes (and the RGB8 plane) are already on the device and nothing is uploaded: the pixel-format entry
 // points of image.cu (include/cvb200_image.h) convert into their own buffers, then take exactly these paths.
+// The capacity reruns of the host calls (akaze.cu): clear the overflow flag before a run; after a run that raised it, grow the
+// keypoint capacities to what the frames needed and set *rerun (CVB_ECAP once `attempt` reaches the limit).
+int akaze_clear_overflow(cvb_ctx *ctx);
+int akaze_capacity_rerun(cvb_ctx *ctx, unsigned B, int attempt, bool *rerun);
 int akaze_extract_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, bool images_on_device, uint32_t batch, uint32_t w,
                              uint32_t h, cvb_keypoint *kp_out, uint8_t *desc_out, uint32_t cap, uint32_t *n_out);
 int frame_features_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const float *images, const uint8_t *rgb, bool planes_on_device,

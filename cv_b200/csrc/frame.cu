@@ -130,17 +130,25 @@ int frame_features_batch_host(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const floa
         CVB_CUDA(ctx, cudaMemcpyAsync(fw->rgb, rgb, 3 * px, cudaMemcpyHostToDevice, st));
         images = fw->img; rgb = fw->rgb;
     }
-    if ((rc = cvb_akaze_extract_batch_dev(ctx, cfg, images, batch, w, h, fw->kp, fw->desc, cd, fw->n))) return rc;
-    if ((rc = cvb_frame_features_batch_dev(ctx, fw->kp, fw->n, batch, cd, rgb, w, h, intrinsics, fw->bear, fw->col))) return rc;
-    // counts behind word 0 of the page-locked scratch, which cvb_akaze_dev_overflow fills with the flag (and then synchronises)
-    uint32_t *hs = (uint32_t *)cvb_pinned(ctx, sizeof(uint32_t) * ((size_t)batch + 1));
-    if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
-    CVB_CUDA(ctx, cudaMemcpyAsync(hs + 1, fw->n, sizeof(uint32_t) * batch, cudaMemcpyDeviceToHost, st));
-    uint32_t ovf = 0;
-    if ((rc = cvb_akaze_dev_overflow(ctx, &ovf))) return rc;
-    for (uint32_t b = 0; b < batch; b++) n_out[b] = hs[1 + b];
-    if (ovf == 3) return cvb_set_error(ctx, CVB_ECAP, "output capacity %u too small", cap);
-    if (ovf) return cvb_set_error(ctx, CVB_ECAP, "internal keypoint capacity exceeded (stage %u)", ovf);
+    // a frame that exceeds the extractor's keypoint capacities is run again in a grown workspace (the planes stay resident)
+    if ((rc = akaze_clear_overflow(ctx))) return rc;
+    for (int attempt = 0;; attempt++) {
+        if ((rc = cvb_akaze_extract_batch_dev(ctx, cfg, images, batch, w, h, fw->kp, fw->desc, cd, fw->n))) return rc;
+        if ((rc = cvb_frame_features_batch_dev(ctx, fw->kp, fw->n, batch, cd, rgb, w, h, intrinsics, fw->bear, fw->col))) return rc;
+        // counts behind word 0 of the page-locked scratch, which cvb_akaze_dev_overflow fills with the flag (and then synchronises)
+        uint32_t *hs = (uint32_t *)cvb_pinned(ctx, sizeof(uint32_t) * ((size_t)batch + 1));
+        if (!hs) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+        CVB_CUDA(ctx, cudaMemcpyAsync(hs + 1, fw->n, sizeof(uint32_t) * batch, cudaMemcpyDeviceToHost, st));
+        uint32_t ovf = 0;
+        if ((rc = cvb_akaze_dev_overflow(ctx, &ovf))) return rc;
+        for (uint32_t b = 0; b < batch; b++) n_out[b] = hs[1 + b];
+        if (!ovf) break;
+        bool rerun = false;
+        if ((rc = akaze_capacity_rerun(ctx, batch, attempt, &rerun))) return rc;
+        if (rerun) continue;
+        if (ovf == 3) return cvb_set_error(ctx, CVB_ECAP, "output capacity %u too small", cap);
+        break;
+    }
     for (uint32_t b = 0; b < batch; b++) {
         const size_t n = std::min<uint32_t>(n_out[b], cap), o = (size_t)b * cap, od = (size_t)b * cd;
         if (!n) continue;

@@ -113,7 +113,16 @@ int cvb_akaze_extract_batch_dev(cvb_ctx *ctx, const cvb_akaze_cfg *cfg, const fl
                                 uint32_t cap, uint32_t *n_out_dev);
 /* The device-resident variant cannot return CVB_ECAP (nothing is read back): n_out_dev never exceeds cap, and a truncation
  * sets a sticky flag.  This call synchronises the stream, returns the flag (0 none, 1/2 internal candidate / keypoint capacity,
- * 3 output capacity) of the extract calls since the last query and clears it. */
+ * 3 output capacity) of the extract calls since the last query and clears it.
+ * Internal capacities: the context's workspace holds max(w*h/8, 4096) candidates and max(w*h/32, 4096) cached keypoints per frame
+ * (fewer than a frame can need: uniform noise or a threshold near 0 exceeds them).  The host calls (cvb_akaze_extract_batch,
+ * cvb_akaze_extract_dynamic_batch, cvb_akaze_find_image_keypoints, cvb_frame_features_batch and its pixel-format form) then grow
+ * these capacities to what the device counted and run the frames again, at most twice, so they return the reference's keypoints;
+ * the grown capacities stay with the workspace.  A host call clears the flag before it runs and leaves it clear, so a flag it reads
+ * back is its own.  The _dev calls cannot run again: they return the keypoints of the clamped stages and set flag 1 or 2.  Such an
+ * overflow leaves nothing behind that changes a later call: the next call runs on the capacities the workspace has (grown by any
+ * host call in between).  The two-view entry of cvb200_sfm.h, cvb_two_view_frames_k1, runs the extractor as the _dev call does and
+ * reads back no flag. */
 int cvb_akaze_dev_overflow(cvb_ctx *ctx, uint32_t *flag_out);
 
 /* Introspection of the last extract call (parity tests): copies one plane of one evolution of one

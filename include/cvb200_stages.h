@@ -26,8 +26,9 @@
  * already depends on it.  The reference reads them from find_image_keypoints' &self, so a caller must build the scale space with
  * the Akaze it detects with.  n_out[b] is the count.  More
  * than cap keypoints: the host call returns CVB_ECAP with n_out[b] = the required count; the _dev call writes the first cap and
- * sets flag 3 of cvb_akaze_dev_overflow.  Every call runs detection again, so an internal capacity exceeded there is reported by
- * every call (CVB_ECAP from the host call; flag 1 or 2 from the _dev call).  An image too small for one octave (no evolutions)
+ * sets flag 3 of cvb_akaze_dev_overflow.  Every call runs detection again.  When a frame exceeds an internal capacity there, the host
+ * call grows the capacity and detects again on the same planes (the ticket stays valid); the _dev call sets flag 1 or 2 (see
+ * cvb_akaze_dev_overflow in cvb200.h).  An image too small for one octave (no evolutions)
  * gives 0 keypoints.
  *
  * describe: the keypoints of frame b are kp_in[offsets[b] .. offsets[b + 1]) (offsets: batch + 1 non-decreasing entries, CSR).
