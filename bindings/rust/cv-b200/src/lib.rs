@@ -216,3 +216,6 @@ pub mod reconstruction;
 
 // ---- INTEGRATION.md section 2o (include/cvb200_export.h) ----
 pub mod export;
+
+// ---- INTEGRATION.md section 2p (include/cvb200_register.h) ----
+pub mod register;

@@ -28,6 +28,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
   robust_landmarks, normalize_reconstruction, export_reconstruction, ExportSettings <- cv-sfm VSlam::triangulate_landmark_robust /
                            normalize_reconstruction / export_reconstruction (cv-sfm/src/lib.rs:2241-2340, 2907-3000) of one
                            reconstruction snapshot in one call each
+  register_frame, RegisterSettings <- cv-sfm VSlam::register_frame (cv-sfm/src/lib.rs:1452-1812): one new frame against one
+                           reconstruction snapshot, from its descriptors to the refined pose and its landmark matches, in one call
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -58,5 +60,6 @@ from .features import frame_features  # noqa: F401
 from .constraints import ConstraintSettings, generate_view_constraints  # noqa: F401
 from .reconstruction import ReconstructionSettings, optimize_reconstruction, regenerate_reconstruction  # noqa: F401
 from .export import ExportSettings, export_reconstruction, normalize_reconstruction, robust_landmarks  # noqa: F401
+from .register import RegisterSettings, register_frame  # noqa: F401
 
 __version__ = "0.1.0"

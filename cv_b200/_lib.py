@@ -2,8 +2,9 @@
 cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (include/cvb200_pinhole.h), cv_b200/libcvb200_image.so
 (include/cvb200_image.h), cv_b200/libcvb200_filter.so (include/cvb200_filter.h), cv_b200/libcvb200_lsh.so (include/cvb200_lsh.h),
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
-(include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h) and cv_b200/libcvb200_reconstruction.so
-(include/cvb200_reconstruction.h) and cv_b200/libcvb200_export.so (include/cvb200_export.h)."""
+(include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h), cv_b200/libcvb200_reconstruction.so
+(include/cvb200_reconstruction.h), cv_b200/libcvb200_export.so (include/cvb200_export.h) and
+cv_b200/libcvb200_register.so (include/cvb200_register.h)."""
 import ctypes as C
 import os
 
@@ -138,6 +139,9 @@ RECONSTRUCTION_ABI_SYMBOLS = ["cvb_recon_cfg_default", "cvb_optimize_reconstruct
 EXPORT_ABI_SYMBOLS = ["cvb_export_cfg_default", "cvb_export_check", "cvb_robust_landmarks_dev", "cvb_robust_landmarks",
                       "cvb_export_reconstruction_dev", "cvb_export_reconstruction", "cvb_normalize_reconstruction_dev",
                       "cvb_normalize_reconstruction"]
+# every symbol include/cvb200_register.h declares (cv-sfm's frame registration), exported by libcvb200_register.so; checked by
+# tests/test_abi_register.py
+REGISTER_ABI_SYMBOLS = ["cvb_register_cfg_default", "cvb_register_check", "cvb_register_frame_dev", "cvb_register_frame"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -452,6 +456,33 @@ def load_export_library():
         L.cvb_normalize_reconstruction.argtypes = [vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u32, u32, vp, vp, vp]
         _EXPORT_LIB = L
     return _EXPORT_LIB
+
+
+_REGISTER_LIB = None
+
+
+def register_lib_path():
+    return os.path.join(_HERE, "libcvb200_register.so")
+
+
+def load_register_library():
+    """Loads libcvb200_register.so, the module of include/cvb200_register.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _REGISTER_LIB
+    if _REGISTER_LIB is None:
+        load_library()
+        p = register_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_register_cfg_default.argtypes = [vp]
+        L.cvb_register_cfg_default.restype = None
+        L.cvb_register_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32]
+        L.cvb_register_frame_dev.argtypes = [vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, u32, vp, vp, u32, vp, vp, u32, vp, u32, vp, vp,
+                                             vp, vp]
+        L.cvb_register_frame.argtypes = [vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, u32, vp, vp, vp, vp]
+        _REGISTER_LIB = L
+    return _REGISTER_LIB
 
 
 class Context:

@@ -23,6 +23,7 @@
 #include "../../include/cvb200_constraints.h"
 #include "../../include/cvb200_reconstruction.h"
 #include "../../include/cvb200_export.h"
+#include "../../include/cvb200_register.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1577,6 +1578,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 #include "constraints_dev.cuh"
 #include "reconstruction_dev.cuh"
 #include "export_dev.cuh"
+#include "register_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1738,12 +1740,13 @@ struct GeomWorkspace {
     DevBuf con, con2;               // the view constraints' snapshot / per-chunk and per-sub-chunk workspaces (view_constraints_dev)
     DevBuf rec;                     // the reconstruction optimisation's workspace (optimize_reconstruction_dev)
     DevBuf exp;                     // the export's workspace (export_dev.cuh's drivers)
+    DevBuf reg;                     // frame registration's workspace (register_frame_dev)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2, &g->rec, &g->exp};
+                      &g->con2, &g->rec, &g->exp, &g->reg};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -3625,6 +3628,232 @@ int normalize_reconstruction(cvb_ctx *ctx, const cvb_export_cfg *cfg, const cvb_
     CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, o + i_pout, sizeof(cvb_pose) * V, cudaMemcpyDeviceToHost, st));
     if (C) CVB_CUDA(ctx, cudaMemcpyAsync(cons_out, o + i_cout, sizeof(cvb_view_constraint) * (size_t)C, cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cudaMemcpyAsync(res, o + i_res, sizeof(cvb_normalize_result), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+// ---- cv-sfm's frame registration (C names in register_abi.cu, include/cvb200_register.h; kernels in register_dev.cuh) ------------------
+void register_cfg_default(cvb_register_cfg *c) {
+    if (!c) return;
+    memset(c, 0, sizeof(*c));
+    c->single_view_optimization_rate = 1e-3;
+    c->maximum_sine_distance = 0.1;
+    c->maximum_cosine_distance = 1e-5;
+    c->robust_observation_incidence_minimum_cosine_distance = 1e-3;
+    c->single_view_match_better_by = 24;
+    c->single_view_initial_features = 1u << 13;
+    c->single_view_minimum_landmarks = 1u << 5;
+    c->single_view_optimization_num_matches = 1u << 11;
+    c->single_view_filter_loop_iterations = 5;
+    c->single_view_patience = 100000;
+    c->single_view_minimum_robust_landmarks = 1u << 6;
+    c->robust_minimum_observations = 3;
+}
+
+int register_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                   const uint32_t *view_matches, uint32_t H) {
+    return view_constraints_check(V, vo, vl, L, lo, obs, view_matches, H);
+}
+
+int register_frame_dev(cvb_ctx *ctx, const cvb_register_cfg *cfg, const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng,
+                       uint32_t V, const cvb_pose *poses_dev, const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev,
+                       const uint8_t *desc_dev, uint32_t n_features, uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev,
+                       uint32_t n_obs, const uint8_t *new_desc_dev, const double *new_bear_dev, uint32_t N, const uint32_t *view_matches,
+                       uint32_t H, cvb_register_result *res_dev, cvb_register_match *matches_dev, uint32_t *inliers_dev,
+                       cvb_register_stats *stats_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !arrsac || !rng || !poses_dev || !view_off_dev || !lm_off_dev || !res_dev || (H && !view_matches) ||
+        (n_features && (!view_lm_dev || !bear_dev || !desc_dev)) || (n_obs && !obs_dev) ||
+        (N && (!new_desc_dev || !new_bear_dev || !matches_dev)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: registration takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    if (N && cfg->single_view_initial_features == 0)   // the reference's subset range would stay empty forever
+        return cvb_set_error(ctx, CVB_EINVAL, "single_view_initial_features must be > 0");
+    for (uint32_t h = 0; h < H; h++)
+        if (view_matches[h] >= V) return cvb_set_error(ctx, CVB_EINVAL, "view match %u of %u views", view_matches[h], V);
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    // the k-NN needs each matched view's stretch of the descriptors: the view offsets, read back once
+    std::vector<uint32_t> vo(V + 1);
+    CVB_CUDA(ctx, cudaMemcpyAsync(vo.data(), view_off_dev, sizeof(uint32_t) * (V + 1), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (vo[V] != n_features) return cvb_set_error(ctx, CVB_EINVAL, "view_offsets[V] = %u, n_features %u", vo[V], n_features);
+    const uint32_t N1 = std::max<uint32_t>(N, 1), H1 = std::max<uint32_t>(H, 1), n2max = con_pow2(N1);
+    const size_t S = (size_t)n_obs + N1;   // scratch slots: each landmark is in at most one kept match, plus one slot per match
+    const bool sine = tri->method == CVB_TRI_SINE_L1;
+    size_t off = 0;
+    const size_t o_ctl = off; off += con_align(sizeof(RegCtl));
+    const size_t o_idx = off; off += con_align(sizeof(uint32_t) * 3 * (size_t)H1 * N1);
+    const size_t o_dist = off; off += con_align(sizeof(uint32_t) * 3 * (size_t)H1 * N1);
+    const size_t o_vbase = off; off += con_align(sizeof(uint32_t) * H1);
+    const size_t o_dec = off; off += con_align(sizeof(uint2) * N1);
+    const size_t o_orig = off; off += con_align(sizeof(RegMatch) * N1);
+    const size_t o_cnt = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t o_keys = off; off += con_align(sizeof(unsigned long long) * n2max);
+    const size_t o_list = off; off += con_align(sizeof(uint32_t) * N1);
+    const size_t o_soff = off; off += con_align(sizeof(uint32_t) * N1);
+    const size_t o_rob = off; off += con_align(N1);
+    const size_t o_cons = off; off += con_align(N1);
+    const size_t o_fin = off; off += con_align(N1);
+    const size_t o_pt = off; off += con_align(sizeof(double) * 4 * N1);
+    const size_t o_sp = off; off += con_align(sizeof(cvb_pose) * S);
+    const size_t o_sb = off; off += con_align(sizeof(double) * 3 * S);
+    const size_t o_sw = off; off += con_align(sizeof(double) * 3 * S);
+    const size_t o_W = off; off += sine ? con_align(sizeof(double) * 6 * S) : 0;
+    const size_t o_mb = off; off += con_align(sizeof(double) * 3 * N1);
+    const size_t o_mw = off; off += con_align(sizeof(double) * 4 * N1);
+    const size_t o_rb = off; off += con_align(sizeof(double) * 3 * N1);
+    const size_t o_rw = off; off += con_align(sizeof(double) * 4 * N1);
+    const size_t o_inl = off; off += con_align(sizeof(uint32_t) * N1);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->reg.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->reg.p;
+    RegCtl *ctl = (RegCtl *)(b + o_ctl);
+    uint32_t *kidx = (uint32_t *)(b + o_idx), *kdist = (uint32_t *)(b + o_dist), *vbase = (uint32_t *)(b + o_vbase);
+    uint2 *dec = (uint2 *)(b + o_dec);
+    RegMatch *orig = (RegMatch *)(b + o_orig);
+    uint32_t *counts = (uint32_t *)(b + o_cnt), *list = (uint32_t *)(b + o_list), *soff = (uint32_t *)(b + o_soff), *inl = (uint32_t *)(b + o_inl);
+    unsigned long long *keys = (unsigned long long *)(b + o_keys);
+    uint8_t *rob = b + o_rob, *cons = b + o_cons, *fin = b + o_fin;
+    double *pt = (double *)(b + o_pt), *sb = (double *)(b + o_sb), *sw = (double *)(b + o_sw), *W = sine ? (double *)(b + o_W) : nullptr;
+    double *mb = (double *)(b + o_mb), *mw = (double *)(b + o_mw), *rb = (double *)(b + o_rb), *rw = (double *)(b + o_rw);
+    cvb_pose *sp = (cvb_pose *)(b + o_sp);
+    std::vector<uint32_t> hbase(H1, 0);
+    for (uint32_t h = 0; h < H; h++) hbase[h] = vo[view_matches[h]];
+    CVB_CUDA(ctx, cudaMemcpyAsync(vbase, hbase.data(), sizeof(uint32_t) * H1, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemsetAsync(ctl, 0, sizeof(RegCtl), st));
+    CVB_CUDA(ctx, cudaMemsetAsync(rob, 0, N1, st));
+    RegParams prm;
+    prm.max_sin = cfg->maximum_sine_distance;
+    prm.max_cos = cfg->maximum_cosine_distance;
+    prm.inc = cfg->robust_observation_incidence_minimum_cosine_distance;
+    prm.better_by = cfg->single_view_match_better_by;
+    prm.min_obs = std::min(cfg->robust_minimum_observations, V);
+    prm.min_landmarks = cfg->single_view_minimum_landmarks;
+    prm.num_matches = cfg->single_view_optimization_num_matches;
+    prm.iters = cfg->single_view_filter_loop_iterations;
+    prm.min_robust_landmarks = cfg->single_view_minimum_robust_landmarks;
+    uint32_t r0 = 0, r1 = std::min(cfg->single_view_initial_features, N), subset = 0;
+    for (;;) {
+        subset++;
+        const uint32_t n = r1 - r0, n2 = con_pow2(std::max<uint32_t>(r1, 1));
+        {
+            CVB_PROF(ctx, "register_match", 0);
+            k_reg_begin<<<1, 1, 0, st>>>(ctl);
+            CVB_LAUNCH_CHECK(ctx);
+            for (uint32_t hh = 0; hh < H && n; hh++) {
+                const uint32_t v = view_matches[hh], m = vo[v + 1] - vo[v];
+                uint32_t *ki = kidx + 3 * (size_t)hh * n, *kd = kdist + 3 * (size_t)hh * n;
+                if (m == 0) {
+                    CVB_CUDA(ctx, cudaMemsetAsync(ki, 0xff, sizeof(uint32_t) * 3 * (size_t)n, st));
+                    continue;
+                }
+                if ((rc = cvb_hamming_knn_dev(ctx, new_desc_dev + 64 * (size_t)r0, n, desc_dev + 64 * (size_t)vo[v], m, 3, ki, kd))) return rc;
+            }
+            if (n) {
+                k_reg_candidates<<<cdiv(n, 128), 128, 0, st>>>(kidx, kdist, n, H, vbase, view_lm_dev, lm_off_dev, obs_dev, prm.better_by, dec, ctl);
+                CVB_LAUNCH_CHECK(ctx);
+                k_reg_append<<<1, 1024, 0, st>>>(dec, n, r0, orig, ctl);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            if (L) CVB_CUDA(ctx, cudaMemsetAsync(counts, 0, sizeof(uint32_t) * L, st));
+            k_reg_claims<<<cdiv(std::max<uint32_t>(r1, 1), 256), 256, 0, st>>>(orig, ctl, counts);
+            CVB_LAUNCH_CHECK(ctx);
+            k_reg_keys<<<cdiv(n2, 256), 256, 0, st>>>(orig, counts, lm_off_dev, ctl, n2, keys);
+            CVB_LAUNCH_CHECK(ctx);
+            k_reg_order<<<1, 1024, 0, st>>>(keys, n2, orig, lm_off_dev, ctl, list, soff);
+            CVB_LAUNCH_CHECK(ctx);
+            k_reg_gather<<<cdiv(std::max<uint32_t>(r1, 1), 128), 128, 0, st>>>(*tri, prm, ctl, orig, list, soff, poses_dev, view_off_dev, bear_dev,
+                                                                                lm_off_dev, obs_dev, sp, sb, sw, W, pt, rob);
+            CVB_LAUNCH_CHECK(ctx);
+            k_reg_compact<<<1, 1024, 0, st>>>(0, 0, prm, ctl, orig, list, rob, pt, cons, new_bear_dev, mb, mw);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        {
+            CVB_PROF(ctx, "register_consensus", 0);
+            if ((rc = cvb_arrsac_p3p_dev(ctx, arrsac, mb, mw, &ctl->cons_n, std::max<uint32_t>(r1, 1), rng, &ctl->model, inl,
+                                         std::max<uint32_t>(r1, 1), &ctl->n_inl, &ctl->found)))
+                return rc;
+            k_reg_take<<<1, 1024, 0, st>>>(prm, ctl, inl, mb, mw, rb, rw);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        {
+            CVB_PROF(ctx, "register_filter", 0);
+            for (uint32_t it = 0; it <= prm.iters; it++) {
+                k_single_view_opt<<<1, OPT_NT, 0, st>>>(&ctl->pose[it & 1], rb, rw, ctl->opt_off, cfg->single_view_optimization_rate,
+                                                        cfg->single_view_patience, &ctl->pose[(it + 1) & 1], &ctl->opt_upd);
+                CVB_LAUNCH_CHECK(ctx);
+                k_reg_consistent<<<cdiv(std::max<uint32_t>(r1, 1), 128), 128, 0, st>>>(*tri, prm, ctl, (it + 1) & 1, orig, list, soff, lm_off_dev,
+                                                                                        new_bear_dev, sp, sb, W, cons);
+                CVB_LAUNCH_CHECK(ctx);
+                if (it < prm.iters) {
+                    k_reg_compact<<<1, 1024, 0, st>>>(1, it + 1, prm, ctl, orig, list, rob, pt, cons, new_bear_dev, rb, rw);
+                    CVB_LAUNCH_CHECK(ctx);
+                }
+            }
+            k_reg_final<<<1, 1024, 0, st>>>(prm, ctl, (prm.iters + 1) & 1, subset, orig, list, rob, cons, fin, matches_dev, res_dev, stats_dev);
+            CVB_LAUNCH_CHECK(ctx);
+            if (inliers_dev && r1) CVB_CUDA(ctx, cudaMemcpyAsync(inliers_dev, inl, sizeof(uint32_t) * r1, cudaMemcpyDeviceToDevice, st));
+        }
+        RegCtl *h = (RegCtl *)cvb_pinned(ctx, sizeof(RegCtl));
+        if (!h) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+        CVB_CUDA(ctx, cudaMemcpyAsync(h, ctl, sizeof(RegCtl), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        const int status = h->status;
+        // the consensus ran on the reference's side exactly when the subset got past the robust-landmark count; otherwise the device run
+        // (on a count of 0) consumed nothing and is closed without moving the generator, so that no run is left pending
+        const bool ran = status != CVB_REGISTER_PANIC && status != CVB_REGISTER_FEW_ROBUST_LANDMARKS;
+        if ((rc = cvb_arrsac_commit_rng(ctx, ran ? rng : nullptr, nullptr))) return rc;
+        if (status == CVB_REGISTER_OK || status == CVB_REGISTER_PANIC || r1 == N) break;
+        r0 = r1;
+        r1 = (uint32_t)std::min<uint64_t>(2ull * r1, N);
+    }
+    return 0;
+}
+
+int register_frame(cvb_ctx *ctx, const cvb_register_cfg *cfg, const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng,
+                   uint32_t V, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, uint32_t L,
+                   const uint32_t *lo, const uint32_t *obs, const uint8_t *new_desc, const double *new_bear, uint32_t N,
+                   const uint32_t *view_matches, uint32_t H, cvb_register_result *res, cvb_register_match *matches, uint32_t *inliers,
+                   cvb_register_stats *stats) {
+    if (!ctx) return CVB_EINVAL;
+    if (!cfg || !tri || !arrsac || !rng || !poses || !res || (N && (!new_desc || !new_bear || !matches)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (register_check(V, vo, vl, L, lo, obs, view_matches, H)) return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot or view matches");
+    if (vo[V] && (!bear || !desc)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    const uint32_t nf = vo[V];
+    size_t x = 0;
+    const size_t i_desc = x; x += con_align(64 * (size_t)nf);
+    const size_t i_nd = x; x += con_align(64 * (size_t)N);
+    const size_t i_nb = x; x += con_align(sizeof(double) * 3 * (size_t)N);
+    const size_t i_res = x; x += con_align(sizeof(cvb_register_result));
+    const size_t i_m = x; x += con_align(sizeof(cvb_register_match) * (size_t)N);
+    const size_t i_st = x; x += con_align(sizeof(cvb_register_stats));
+    const size_t i_inl = x; x += con_align(sizeof(uint32_t) * (size_t)N);
+    ExpUpload u;
+    unsigned char *b;
+    int rc;
+    if ((rc = export_upload(ctx, V, poses, vo, vl, bear, nullptr, L, lo, obs, nullptr, 0, x, u, b))) return rc;
+    unsigned char *o = b + u.end;
+    cudaStream_t st = ctx->stream;
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(o + i_desc, desc, 64 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    if (N) CVB_CUDA(ctx, cudaMemcpyAsync(o + i_nd, new_desc, 64 * (size_t)N, cudaMemcpyHostToDevice, st));
+    if (N) CVB_CUDA(ctx, cudaMemcpyAsync(o + i_nb, new_bear, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, st));
+    if ((rc = register_frame_dev(ctx, cfg, tri, arrsac, rng, V, (const cvb_pose *)(b + u.pose), (const uint32_t *)(b + u.vo),
+                                 (const uint32_t *)(b + u.vl), (const double *)(b + u.bear), o + i_desc, nf, L, (const uint32_t *)(b + u.lo),
+                                 (const uint32_t *)(b + u.obs), lo[L], o + i_nd, (const double *)(o + i_nb), N, view_matches, H,
+                                 (cvb_register_result *)(o + i_res), (cvb_register_match *)(o + i_m), inliers ? (uint32_t *)(o + i_inl) : nullptr,
+                                 stats ? (cvb_register_stats *)(o + i_st) : nullptr)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, o + i_res, sizeof(cvb_register_result), cudaMemcpyDeviceToHost, st));
+    if (stats) CVB_CUDA(ctx, cudaMemcpyAsync(stats, o + i_st, sizeof(cvb_register_stats), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (res->n_matches) CVB_CUDA(ctx, cudaMemcpyAsync(matches, o + i_m, sizeof(cvb_register_match) * (size_t)res->n_matches, cudaMemcpyDeviceToHost, st));
+    if (inliers && res->n_inliers) CVB_CUDA(ctx, cudaMemcpyAsync(inliers, o + i_inl, sizeof(uint32_t) * (size_t)res->n_inliers, cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
 }
