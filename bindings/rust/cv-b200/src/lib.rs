@@ -219,3 +219,6 @@ pub mod export;
 
 // ---- INTEGRATION.md section 2p (include/cvb200_register.h) ----
 pub mod register;
+
+// ---- INTEGRATION.md section 2q (include/cvb200_incorporate.h) ----
+pub mod incorporate;

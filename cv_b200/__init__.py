@@ -30,6 +30,9 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
                            reconstruction snapshot in one call each
   register_frame, RegisterSettings <- cv-sfm VSlam::register_frame (cv-sfm/src/lib.rs:1452-1812): one new frame against one
                            reconstruction snapshot, from its descriptors to the refined pose and its landmark matches, in one call
+  add_view, apply_optimization, incorporate_frame <- cv-sfm VSlamData::add_view / merge_landmarks, the remove_view / split_observation
+                           edits of optimize_reconstruction, and VSlam::incorporate_frame followed by optimize_reconstruction
+                           (cv-sfm/src/lib.rs:432-588, 699-721, 2067-2087): one reconstruction snapshot to the next, on the device
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -61,5 +64,6 @@ from .constraints import ConstraintSettings, generate_view_constraints  # noqa: 
 from .reconstruction import ReconstructionSettings, optimize_reconstruction, regenerate_reconstruction  # noqa: F401
 from .export import ExportSettings, export_reconstruction, normalize_reconstruction, robust_landmarks  # noqa: F401
 from .register import RegisterSettings, register_frame  # noqa: F401
+from .incorporate import add_view, apply_optimization, incorporate_frame  # noqa: F401
 
 __version__ = "0.1.0"

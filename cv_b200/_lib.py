@@ -4,7 +4,7 @@ cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (i
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
 (include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h), cv_b200/libcvb200_reconstruction.so
 (include/cvb200_reconstruction.h), cv_b200/libcvb200_export.so (include/cvb200_export.h) and
-cv_b200/libcvb200_register.so (include/cvb200_register.h)."""
+cv_b200/libcvb200_register.so (include/cvb200_register.h) and cv_b200/libcvb200_incorporate.so (include/cvb200_incorporate.h)."""
 import ctypes as C
 import os
 
@@ -142,6 +142,10 @@ EXPORT_ABI_SYMBOLS = ["cvb_export_cfg_default", "cvb_export_check", "cvb_robust_
 # every symbol include/cvb200_register.h declares (cv-sfm's frame registration), exported by libcvb200_register.so; checked by
 # tests/test_abi_register.py
 REGISTER_ABI_SYMBOLS = ["cvb_register_cfg_default", "cvb_register_check", "cvb_register_frame_dev", "cvb_register_frame"]
+# every symbol include/cvb200_incorporate.h declares (cv-sfm's frame incorporation), exported by libcvb200_incorporate.so; checked by
+# tests/test_abi_incorporate.py
+INCORPORATE_ABI_SYMBOLS = ["cvb_incorporate_check", "cvb_add_view_dev", "cvb_add_view", "cvb_apply_optimization_dev", "cvb_apply_optimization",
+                           "cvb_incorporate_frame_dev", "cvb_incorporate_frame"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -483,6 +487,36 @@ def load_register_library():
         L.cvb_register_frame.argtypes = [vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp, u32, vp, u32, vp, vp, vp, vp]
         _REGISTER_LIB = L
     return _REGISTER_LIB
+
+
+_INCORPORATE_LIB = None
+
+
+def incorporate_lib_path():
+    return os.path.join(_HERE, "libcvb200_incorporate.so")
+
+
+def load_incorporate_library():
+    """Loads libcvb200_incorporate.so, the module of include/cvb200_incorporate.h over libcvb200.so (same contexts). Fails loudly when
+    missing."""
+    global _INCORPORATE_LIB
+    if _INCORPORATE_LIB is None:
+        load_library()
+        p = incorporate_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_incorporate_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32, u32, vp, u32, vp, u32, vp, u32]
+        L.cvb_add_view_dev.argtypes = [vp, u32] + [vp] * 6 + [u32, u32, vp, vp, u32] + [vp] * 4 + [u32, vp, u32] + [vp] * 10
+        L.cvb_add_view.argtypes = [vp, u32] + [vp] * 6 + [u32, vp, vp] + [vp] * 4 + [u32, vp, u32] + [vp] * 10
+        L.cvb_apply_optimization_dev.argtypes = [vp, u32] + [vp] * 6 + [u32, u32, vp, vp, u32, vp, u32] + [vp] * 14
+        L.cvb_apply_optimization.argtypes = [vp, u32] + [vp] * 6 + [u32, vp, vp, vp, u32] + [vp] * 14
+        L.cvb_incorporate_frame_dev.argtypes = ([vp] * 7 + [u32] + [vp] * 6 + [u32, u32, vp, vp, u32, vp, u32, vp, vp, vp, u32, vp, u32] +
+                                                [vp] * 13)
+        L.cvb_incorporate_frame.argtypes = [vp] * 7 + [u32] + [vp] * 6 + [u32, vp, vp, vp, u32, vp, vp, vp, u32, vp, u32] + [vp] * 13
+        _INCORPORATE_LIB = L
+    return _INCORPORATE_LIB
 
 
 class Context:

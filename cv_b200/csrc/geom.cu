@@ -24,6 +24,7 @@
 #include "../../include/cvb200_reconstruction.h"
 #include "../../include/cvb200_export.h"
 #include "../../include/cvb200_register.h"
+#include "../../include/cvb200_incorporate.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1579,6 +1580,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 #include "reconstruction_dev.cuh"
 #include "export_dev.cuh"
 #include "register_dev.cuh"
+#include "incorporate_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1741,12 +1743,13 @@ struct GeomWorkspace {
     DevBuf rec;                     // the reconstruction optimisation's workspace (optimize_reconstruction_dev)
     DevBuf exp;                     // the export's workspace (export_dev.cuh's drivers)
     DevBuf reg;                     // frame registration's workspace (register_frame_dev)
+    DevBuf inc, incs;               // frame incorporation's snapshot after add_view and the two edits' scratch (incorporate_frame_dev)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2, &g->rec, &g->exp, &g->reg};
+                      &g->con2, &g->rec, &g->exp, &g->reg, &g->inc, &g->incs};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -3856,6 +3859,674 @@ int register_frame(cvb_ctx *ctx, const cvb_register_cfg *cfg, const cvb_triangul
     if (inliers && res->n_inliers) CVB_CUDA(ctx, cudaMemcpyAsync(inliers, o + i_inl, sizeof(uint32_t) * (size_t)res->n_inliers, cudaMemcpyDeviceToHost, st));
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     return 0;
+}
+
+// ---- cv-sfm's frame incorporation (C names in incorporate_abi.cu, include/cvb200_incorporate.h; kernels in incorporate_dev.cuh) ---------
+int incorporate_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                      const cvb_view_constraint *cons, uint32_t C, uint32_t N, const cvb_register_match *matches, uint32_t M,
+                      const uint8_t *view_state, uint32_t n_view_state, const uint8_t *obs_state, uint32_t n_obs_state) {
+    if (optimize_reconstruction_check(V, vo, vl, L, lo, obs, cons, C)) return CVB_EINVAL;
+    if (M && !matches) return CVB_EINVAL;
+    if (M) {
+        std::vector<uint8_t> used(L, 0);
+        for (uint32_t m = 0; m < M; m++) {
+            const cvb_register_match &t = matches[m];
+            if (t.feature >= N || (m && t.feature <= matches[m - 1].feature)) return CVB_EINVAL;
+            if (t.landmark_a >= L || used[t.landmark_a]) return CVB_EINVAL;
+            used[t.landmark_a] = 1;
+            if (t.landmark_b == CVB_REGISTER_NONE) continue;
+            if (t.landmark_b >= L || t.landmark_b == t.landmark_a || used[t.landmark_b]) return CVB_EINVAL;
+            used[t.landmark_b] = 1;
+            for (uint32_t i = lo[t.landmark_a]; i < lo[t.landmark_a + 1]; i++)   // merge_landmarks' assert!: the two share no view
+                for (uint32_t j = lo[t.landmark_b]; j < lo[t.landmark_b + 1]; j++)
+                    if (obs[2 * (size_t)i] == obs[2 * (size_t)j]) return CVB_EINVAL;
+        }
+    }
+    if (view_state || obs_state) {
+        if (!view_state || n_view_state != V || n_obs_state != lo[L] || (lo[L] && !obs_state)) return CVB_EINVAL;
+        for (uint32_t v = 0; v < V; v++)
+            if (view_state[v] > CVB_RECON_VIEW_NON_FINITE) return CVB_EINVAL;
+        for (uint32_t o = 0; o < lo[L]; o++) {
+            if (obs_state[o] > CVB_RECON_OBS_DROPPED) return CVB_EINVAL;
+            if ((obs_state[o] == CVB_RECON_OBS_DROPPED) != (view_state[obs[2 * (size_t)o]] != CVB_RECON_VIEW_KEPT)) return CVB_EINVAL;
+        }
+        for (uint32_t l = 0; l < L; l++) {   // split_observation never splits a landmark's last observation
+            uint32_t rest = 0;
+            for (uint32_t o = lo[l]; o < lo[l + 1]; o++) rest += obs_state[o] != CVB_RECON_OBS_SPLIT;
+            if (lo[l + 1] > lo[l] && rest == 0) return CVB_EINVAL;
+        }
+    }
+    return 0;
+}
+
+namespace {
+
+// exclusive scan of n pairs in place, the total into *total; tiles: cdiv(n, INC_TILE) pairs of scratch
+int inc_scan(cvb_ctx *ctx, uint32_t n, uint2 *a, uint2 *tiles, uint2 *total) {
+    cudaStream_t st = ctx->stream;
+    const uint32_t nt = cdiv(n, INC_TILE);
+    if (nt) {
+        k_inc_tile_sums<<<nt, INC_NT, 0, st>>>(n, a, tiles);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    k_inc_scan_tiles<<<1, INC_NT, 0, st>>>(nt, tiles, total);
+    CVB_LAUNCH_CHECK(ctx);
+    if (nt) {
+        k_inc_scan_apply<<<nt, INC_NT, 0, st>>>(n, a, tiles);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    return 0;
+}
+
+// the checks every entry makes of the snapshot sizes against the device (one read-back of view_offsets[V] and landmark_offsets[L])
+int inc_sizes(cvb_ctx *ctx, uint32_t V, const uint32_t *view_off_dev, uint32_t n_features, uint32_t L, const uint32_t *lm_off_dev,
+              uint32_t n_obs) {
+    uint32_t *h = (uint32_t *)cvb_pinned(ctx, 2 * sizeof(uint32_t));
+    if (!h) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(h, view_off_dev + V, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cudaMemcpyAsync(h + 1, lm_off_dev + L, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    if (h[0] != n_features) return cvb_set_error(ctx, CVB_EINVAL, "view_offsets[V] = %u, n_features %u", h[0], n_features);
+    if (h[1] != n_obs) return cvb_set_error(ctx, CVB_EINVAL, "landmark_offsets[L] = %u, n_observations %u", h[1], n_obs);
+    return 0;
+}
+
+// add_view, enqueued on the context's stream (no wait); scratch in the context's incorporate scratch buffer
+int add_view_enqueue(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses_dev, const uint32_t *view_off_dev, const uint32_t *view_lm_dev,
+                     const double *bear_dev, const uint8_t *desc_dev, const uint8_t *col_dev, uint32_t nf, uint32_t L, const uint32_t *lm_off_dev,
+                     const uint32_t *obs_dev, uint32_t n_obs, const cvb_pose *new_pose_dev, const double *new_bear_dev, const uint8_t *new_desc_dev,
+                     const uint8_t *new_col_dev, uint32_t N, const cvb_register_match *matches_dev, uint32_t M, cvb_pose *poses_out,
+                     uint32_t *view_off_out, uint32_t *view_lm_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lm_off_out,
+                     uint32_t *obs_out, uint32_t *lmap, cvb_incorporate_counts *counts) {
+    const uint32_t n = L + N, nt = cdiv(n, INC_TILE);
+    size_t off = 0;
+    const size_t o_role = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t o_featm = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(N, 1));
+    const size_t o_merges = off; off += con_align(sizeof(uint32_t));
+    const size_t o_cnt = off; off += con_align(sizeof(uint2) * std::max<size_t>(n, 1));
+    const size_t o_tiles = off; off += con_align(sizeof(uint2) * std::max<size_t>(nt, 1));
+    const size_t o_total = off; off += con_align(sizeof(uint2));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->incs.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->incs.p;
+    uint32_t *role = (uint32_t *)(b + o_role), *featm = (uint32_t *)(b + o_featm), *merges = (uint32_t *)(b + o_merges);
+    uint2 *cnt = (uint2 *)(b + o_cnt), *tiles = (uint2 *)(b + o_tiles), *total = (uint2 *)(b + o_total);
+    cudaStream_t st = ctx->stream;
+    CVB_PROF(ctx, "k_av", 0);
+    CVB_CUDA(ctx, cudaMemsetAsync(b, 0xff, o_merges, st));   // role and featm: INC_NONE
+    CVB_CUDA(ctx, cudaMemsetAsync(merges, 0, sizeof(uint32_t), st));
+    if (M) {
+        k_av_roles<<<cdiv(M, 256), 256, 0, st>>>(M, matches_dev, L, N, role, featm, merges);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (n) {
+        k_av_counts<<<cdiv(n, 256), 256, 0, st>>>(L, N, n_obs, lm_off_dev, role, featm, matches_dev, cnt);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if ((rc = inc_scan(ctx, n, cnt, tiles, total))) return rc;
+    if (n) {
+        k_av_place<<<cdiv(n, 256), 256, 0, st>>>(V, L, N, n_obs, lm_off_dev, obs_dev, role, featm, matches_dev, cnt, n, n_obs + N, lm_off_out,
+                                                 obs_out, lmap);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (nf + N) {
+        k_av_features<<<cdiv(nf + N, 256), 256, 0, st>>>(nf, L, N, view_lm_dev, lmap, featm, matches_dev, cnt, view_lm_out);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    // the rows that only move: poses, view offsets, bearings, descriptors and colours, the new view's after the old ones
+    CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, poses_dev, sizeof(cvb_pose) * V, cudaMemcpyDeviceToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(poses_out + V, new_pose_dev, sizeof(cvb_pose), cudaMemcpyDeviceToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(view_off_out, view_off_dev, sizeof(uint32_t) * (V + 1), cudaMemcpyDeviceToDevice, st));
+    if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(bear_out, bear_dev, sizeof(double) * 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+    if (N) CVB_CUDA(ctx, cudaMemcpyAsync(bear_out + 3 * (size_t)nf, new_bear_dev, sizeof(double) * 3 * (size_t)N, cudaMemcpyDeviceToDevice, st));
+    if (desc_out) {
+        if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(desc_out, desc_dev, 64 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+        if (N) CVB_CUDA(ctx, cudaMemcpyAsync(desc_out + 64 * (size_t)nf, new_desc_dev, 64 * (size_t)N, cudaMemcpyDeviceToDevice, st));
+    }
+    if (col_out) {
+        if (nf) CVB_CUDA(ctx, cudaMemcpyAsync(col_out, col_dev, 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+        if (N) CVB_CUDA(ctx, cudaMemcpyAsync(col_out + 3 * (size_t)nf, new_col_dev, 3 * (size_t)N, cudaMemcpyDeviceToDevice, st));
+    }
+    k_av_finish<<<1, 1, 0, st>>>(V, nf, N, total, merges, n, view_off_out, lm_off_out, counts);
+    CVB_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+// apply_optimization, enqueued on the context's stream (no wait); scratch in the context's incorporate scratch buffer
+int apply_enqueue(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses_dev, const uint32_t *view_off_dev, const double *bear_dev,
+                  const uint8_t *desc_dev, const uint8_t *col_dev, uint32_t nf, uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev,
+                  uint32_t n_obs, const cvb_view_constraint *cons_dev, uint32_t C, const uint8_t *vstate, const uint8_t *ostate,
+                  cvb_pose *poses_out, uint32_t *view_off_out, uint32_t *view_lm_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out,
+                  uint32_t *lm_off_out, uint32_t *obs_out, cvb_view_constraint *cons_out, uint32_t *vmap, uint32_t *lmap,
+                  cvb_incorporate_counts *counts) {
+    const uint32_t nmax = std::max(std::max(V, L), std::max(n_obs, C));
+    size_t off = 0;
+    const size_t o_v = off; off += con_align(sizeof(uint2) * std::max<size_t>(V, 1));
+    const size_t o_l = off; off += con_align(sizeof(uint2) * std::max<size_t>(L, 1));
+    const size_t o_s = off; off += con_align(sizeof(uint2) * std::max<size_t>(n_obs, 1));
+    const size_t o_c = off; off += con_align(sizeof(uint2) * std::max<size_t>(C, 1));
+    const size_t o_tiles = off; off += con_align(sizeof(uint2) * std::max<size_t>(cdiv(nmax, INC_TILE), 1));
+    const size_t o_tot = off; off += con_align(sizeof(uint2) * 4);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->incs.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->incs.p;
+    uint2 *vcnt = (uint2 *)(b + o_v), *lcnt = (uint2 *)(b + o_l), *scnt = (uint2 *)(b + o_s), *ccnt = (uint2 *)(b + o_c);
+    uint2 *tiles = (uint2 *)(b + o_tiles), *tot = (uint2 *)(b + o_tot);
+    cudaStream_t st = ctx->stream;
+    CVB_PROF(ctx, "k_ap", 0);
+    k_ap_view_counts<<<cdiv(V, 256), 256, 0, st>>>(V, nf, view_off_dev, vstate, vcnt);
+    CVB_LAUNCH_CHECK(ctx);
+    if ((rc = inc_scan(ctx, V, vcnt, tiles, tot + 0))) return rc;
+    if (L) {
+        k_ap_landmark_counts<<<cdiv(L, 256), 256, 0, st>>>(L, n_obs, lm_off_dev, ostate, lcnt);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if ((rc = inc_scan(ctx, L, lcnt, tiles, tot + 1))) return rc;
+    if (n_obs) {
+        k_ap_split_counts<<<cdiv(n_obs, 256), 256, 0, st>>>(n_obs, ostate, scnt);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if ((rc = inc_scan(ctx, n_obs, scnt, tiles, tot + 2))) return rc;
+    if (C) {
+        k_ap_constraint_counts<<<cdiv(C, 256), 256, 0, st>>>(C, V, cons_dev, vstate, ccnt);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if ((rc = inc_scan(ctx, C, ccnt, tiles, tot + 3))) return rc;
+    k_ap_views<<<cdiv(V, 256), 256, 0, st>>>(V, poses_dev, vstate, vcnt, poses_out, view_off_out, vmap);
+    CVB_LAUNCH_CHECK(ctx);
+    k_ap_feature_rows<<<cdiv(V * 32, 256), 256, 0, st>>>(V, nf, view_off_dev, vstate, vcnt, bear_dev, (const uint4 *)desc_dev, col_dev, bear_out,
+                                                         (uint4 *)desc_out, col_out);
+    CVB_LAUNCH_CHECK(ctx);
+    if (L) {
+        k_ap_landmarks<<<cdiv(L, 256), 256, 0, st>>>(V, nf, L, n_obs, view_off_dev, vstate, vcnt, lm_off_dev, obs_dev, ostate, lcnt, tot + 1,
+                                                     lm_off_out, obs_out, view_lm_out, lmap);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (n_obs) {
+        k_ap_splits<<<cdiv(n_obs, 256), 256, 0, st>>>(V, nf, L, n_obs, view_off_dev, vstate, vcnt, obs_dev, ostate, scnt, tot + 1, lm_off_out,
+                                                      obs_out, view_lm_out);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (C) {
+        k_ap_constraints<<<cdiv(C, 256), 256, 0, st>>>(C, cons_dev, ccnt, tot + 3, vcnt, cons_out);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    k_ap_finish<<<1, 1, 0, st>>>(tot + 0, tot + 1, tot + 2, tot + 3, L + n_obs, view_off_out, lm_off_out, counts);
+    CVB_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+}  // namespace
+
+int add_view_dev(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses_dev, const uint32_t *view_off_dev, const uint32_t *view_lm_dev,
+                 const double *bear_dev, const uint8_t *desc_dev, const uint8_t *col_dev, uint32_t nf, uint32_t L, const uint32_t *lm_off_dev,
+                 const uint32_t *obs_dev, uint32_t n_obs, const cvb_pose *new_pose_dev, const double *new_bear_dev, const uint8_t *new_desc_dev,
+                 const uint8_t *new_col_dev, uint32_t N, const cvb_register_match *matches_dev, uint32_t M, cvb_pose *poses_out,
+                 uint32_t *view_off_out, uint32_t *view_lm_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lm_off_out,
+                 uint32_t *obs_out, uint32_t *lmap, cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!poses_dev || !view_off_dev || !lm_off_dev || !new_pose_dev || !poses_out || !view_off_out || !lm_off_out || !counts ||
+        (nf && (!view_lm_dev || !bear_dev)) || (n_obs && !obs_dev) || (N && !new_bear_dev) || (M && !matches_dev) ||
+        (nf + N && (!view_lm_out || !bear_out)) || (n_obs + N && !obs_out) || (L && !lmap))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    // descriptors and colours: the snapshot's, the new frame's and the output all given or all omitted
+    if ((nf && (!desc_dev != !desc_out)) || (N && (!new_desc_dev != !desc_out)) || (nf && (!col_dev != !col_out)) ||
+        (N && (!new_col_dev != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with the snapshot, the new frame and the output together");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = inc_sizes(ctx, V, view_off_dev, nf, L, lm_off_dev, n_obs))) return rc;
+    if ((rc = add_view_enqueue(ctx, V, poses_dev, view_off_dev, view_lm_dev, bear_dev, desc_dev, col_dev, nf, L, lm_off_dev, obs_dev, n_obs,
+                               new_pose_dev, new_bear_dev, new_desc_dev, new_col_dev, N, matches_dev, M, poses_out, view_off_out, view_lm_out,
+                               bear_out, desc_out, col_out, lm_off_out, obs_out, lmap, counts)))
+        return rc;
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int apply_optimization_dev(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses_dev, const uint32_t *view_off_dev, const uint32_t *view_lm_dev,
+                           const double *bear_dev, const uint8_t *desc_dev, const uint8_t *col_dev, uint32_t nf, uint32_t L,
+                           const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs, const cvb_view_constraint *cons_dev, uint32_t C,
+                           const uint8_t *vstate, const uint8_t *ostate, cvb_pose *poses_out, uint32_t *view_off_out, uint32_t *view_lm_out,
+                           double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lm_off_out, uint32_t *obs_out,
+                           cvb_view_constraint *cons_out, uint32_t *vmap, uint32_t *lmap, cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!poses_dev || !view_off_dev || !lm_off_dev || !poses_out || !view_off_out || !lm_off_out || !counts ||
+        (nf && (!view_lm_dev || !bear_dev || !view_lm_out || !bear_out)) || (n_obs && (!obs_dev || !ostate || !obs_out)) ||
+        (C && (!cons_dev || !cons_out)) || (V && (!vstate || !vmap)) || (L && !lmap))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (nf && ((!desc_dev != !desc_out) || (!col_dev != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with the snapshot and the output together");
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = inc_sizes(ctx, V, view_off_dev, nf, L, lm_off_dev, n_obs))) return rc;
+    if ((rc = apply_enqueue(ctx, V, poses_dev, view_off_dev, bear_dev, desc_dev, col_dev, nf, L, lm_off_dev, obs_dev, n_obs, cons_dev, C, vstate,
+                            ostate, poses_out, view_off_out, view_lm_out, bear_out, desc_out, col_out, lm_off_out, obs_out, cons_out, vmap, lmap,
+                            counts)))
+        return rc;
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+namespace {
+
+// device rows of one snapshot with the given capacities, carved out of one buffer
+struct IncSnap {
+    cvb_pose *poses; uint32_t *vo, *vl; double *bear; uint8_t *desc, *col; uint32_t *lo, *obs; cvb_view_constraint *cons;
+};
+size_t inc_snap_layout(size_t base, uint32_t V, uint32_t nf, uint32_t L, uint32_t n_obs, uint32_t C, bool desc, bool col, size_t *o) {
+    size_t off = base;
+    o[0] = off; off += con_align(sizeof(cvb_pose) * std::max<size_t>(V, 1));
+    o[1] = off; off += con_align(sizeof(uint32_t) * ((size_t)V + 1));
+    o[2] = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(nf, 1));
+    o[3] = off; off += con_align(sizeof(double) * 3 * std::max<size_t>(nf, 1));
+    o[4] = off; off += desc ? con_align(64 * std::max<size_t>(nf, 1)) : 0;
+    o[5] = off; off += col ? con_align(3 * std::max<size_t>(nf, 1)) : 0;
+    o[6] = off; off += con_align(sizeof(uint32_t) * ((size_t)L + 1));
+    o[7] = off; off += con_align(sizeof(uint32_t) * 2 * std::max<size_t>(n_obs, 1));
+    o[8] = off; off += con_align(sizeof(cvb_view_constraint) * std::max<size_t>(C, 1));
+    return off;
+}
+IncSnap inc_snap_at(unsigned char *b, const size_t *o, bool desc, bool col) {
+    IncSnap s;
+    s.poses = (cvb_pose *)(b + o[0]);
+    s.vo = (uint32_t *)(b + o[1]);
+    s.vl = (uint32_t *)(b + o[2]);
+    s.bear = (double *)(b + o[3]);
+    s.desc = desc ? b + o[4] : nullptr;
+    s.col = col ? b + o[5] : nullptr;
+    s.lo = (uint32_t *)(b + o[6]);
+    s.obs = (uint32_t *)(b + o[7]);
+    s.cons = (cvb_view_constraint *)(b + o[8]);
+    return s;
+}
+
+}  // namespace
+
+int incorporate_frame_dev(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_constraints_cfg *ccfg, const cvb_recon_cfg *ocfg,
+                          const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng, uint32_t V, const cvb_pose *poses_dev,
+                          const uint32_t *view_off_dev, const uint32_t *view_lm_dev, const double *bear_dev, const uint8_t *desc_dev,
+                          const uint8_t *col_dev, uint32_t nf, uint32_t L, const uint32_t *lm_off_dev, const uint32_t *obs_dev, uint32_t n_obs,
+                          const cvb_view_constraint *cons_dev, uint32_t C, const uint8_t *new_desc_dev, const double *new_bear_dev,
+                          const uint8_t *new_col_dev, uint32_t N, const uint32_t *view_matches, uint32_t H, cvb_pose *poses_out,
+                          uint32_t *view_off_out, uint32_t *view_lm_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out,
+                          uint32_t *lm_off_out, uint32_t *obs_out, cvb_view_constraint *cons_out, uint32_t *vmap, uint32_t *lmap,
+                          cvb_register_match *matches_out, cvb_incorporate_result *res_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!rcfg || !ccfg || !ocfg || !tri || !arrsac || !rng || !poses_dev || !view_off_dev || !lm_off_dev || !res_dev || !poses_out ||
+        !view_off_out || !lm_off_out || (H && !view_matches) || (nf && (!view_lm_dev || !bear_dev || !desc_dev)) || (n_obs && !obs_dev) ||
+        (C && !cons_dev) || (N && (!new_desc_dev || !new_bear_dev)) || (nf + N && (!view_lm_out || !bear_out || !desc_out)) ||
+        (n_obs + N && !obs_out) || (V && !vmap) || (L && !lmap) || !cons_out)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!col_dev != !col_out)) || (N && (!new_col_dev != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "colours go with the snapshot, the new frame and the output together");
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: incorporation takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (ccfg->optimization_maximum_landmarks > CVB_CONSTRAINTS_MAX_LANDMARKS)
+        return cvb_set_error(ctx, CVB_EUNSUPPORTED, "optimization_maximum_landmarks %u > %u", ccfg->optimization_maximum_landmarks,
+                             CVB_CONSTRAINTS_MAX_LANDMARKS);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = inc_sizes(ctx, V, view_off_dev, nf, L, lm_off_dev, n_obs))) return rc;
+    cudaStream_t st = ctx->stream;
+    const bool col = col_out != nullptr;
+    const uint32_t maxc = ccfg->optimization_maximum_three_view_constraints;
+    const uint32_t V1 = V + 1, nf1 = nf + N, L1 = L + N, no1 = n_obs + N, C1 = C + maxc;
+    // the workspace: register's outputs, the snapshot after add_view (with room for the new constraints after the old ones), the
+    // optimisation's outputs and the maps of the two edits
+    size_t o[9], off = 0;
+    const size_t o_rres = off; off += con_align(sizeof(cvb_register_result));
+    const size_t o_rst = off; off += con_align(sizeof(cvb_register_stats));
+    const size_t o_m = off; off += con_align(sizeof(cvb_register_match) * std::max<size_t>(N, 1));
+    const size_t o_cres = off; off += con_align(sizeof(cvb_view_constraints_result));
+    const size_t o_ores = off; off += con_align(sizeof(cvb_recon_result));
+    const size_t o_cnt = off; off += con_align(sizeof(cvb_incorporate_counts) * 2);
+    const size_t o_pout = off; off += con_align(sizeof(cvb_pose) * V1);
+    const size_t o_vs = off; off += con_align(V1);
+    const size_t o_os = off; off += con_align(std::max<size_t>(no1, 1));
+    const size_t o_amap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t o_vmap = off; off += con_align(sizeof(uint32_t) * V1);
+    const size_t o_lmap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L1, 1));
+    off = inc_snap_layout(off, V1, nf1, L1, no1, C1, true, col, o);
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = g->inc.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->inc.p;
+    cvb_register_result *rres = (cvb_register_result *)(b + o_rres);
+    cvb_register_stats *rst = (cvb_register_stats *)(b + o_rst);
+    cvb_register_match *mt = (cvb_register_match *)(b + o_m);
+    cvb_view_constraints_result *cres = (cvb_view_constraints_result *)(b + o_cres);
+    cvb_recon_result *ores = (cvb_recon_result *)(b + o_ores);
+    cvb_incorporate_counts *cnt = (cvb_incorporate_counts *)(b + o_cnt);
+    cvb_pose *pout = (cvb_pose *)(b + o_pout);
+    uint8_t *vs = b + o_vs, *os = b + o_os;
+    uint32_t *amap = (uint32_t *)(b + o_amap), *avmap = (uint32_t *)(b + o_vmap), *almap = (uint32_t *)(b + o_lmap);
+    IncSnap a = inc_snap_at(b, o, true, col);
+    cvb_incorporate_result R;
+    memset(&R, 0, sizeof(R));
+    R.new_view = CVB_INCORPORATE_NONE;
+    // 1. register_frame
+    if ((rc = register_frame_dev(ctx, rcfg, tri, arrsac, rng, V, poses_dev, view_off_dev, view_lm_dev, bear_dev, desc_dev, nf, L, lm_off_dev,
+                                 obs_dev, n_obs, new_desc_dev, new_bear_dev, N, view_matches, H, rres, mt, nullptr, rst)))
+        return rc;
+    std::vector<cvb_register_match> hm;
+    {
+        CVB_CUDA(ctx, cudaMemcpyAsync(&R.reg, rres, sizeof(cvb_register_result), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(&R.reg_stats, rst, sizeof(cvb_register_stats), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+    }
+    const uint32_t M = R.reg.status == CVB_REGISTER_OK ? R.reg.n_matches : 0;
+    if (matches_out && M) CVB_CUDA(ctx, cudaMemcpyAsync(matches_out, mt, sizeof(cvb_register_match) * M, cudaMemcpyDeviceToDevice, st));
+    bool have = false;            // an output snapshot exists
+    bool edited = false;          // ... and it came through the apply step (maps composed from add_view's and apply's)
+    if (R.reg.status == CVB_REGISTER_PANIC) {
+        R.status = CVB_INCORPORATE_REGISTER_PANIC;
+    } else if (R.reg.status != CVB_REGISTER_OK) {
+        // the input, unchanged
+        R.status = CVB_INCORPORATE_NOT_REGISTERED;
+        CVB_CUDA(ctx, cudaMemcpyAsync(poses_out, poses_dev, sizeof(cvb_pose) * V, cudaMemcpyDeviceToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(view_off_out, view_off_dev, sizeof(uint32_t) * (V + 1), cudaMemcpyDeviceToDevice, st));
+        if (nf) {
+            CVB_CUDA(ctx, cudaMemcpyAsync(view_lm_out, view_lm_dev, sizeof(uint32_t) * nf, cudaMemcpyDeviceToDevice, st));
+            CVB_CUDA(ctx, cudaMemcpyAsync(bear_out, bear_dev, sizeof(double) * 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+            CVB_CUDA(ctx, cudaMemcpyAsync(desc_out, desc_dev, 64 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+            if (col) CVB_CUDA(ctx, cudaMemcpyAsync(col_out, col_dev, 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+        }
+        CVB_CUDA(ctx, cudaMemcpyAsync(lm_off_out, lm_off_dev, sizeof(uint32_t) * ((size_t)L + 1), cudaMemcpyDeviceToDevice, st));
+        if (n_obs) CVB_CUDA(ctx, cudaMemcpyAsync(obs_out, obs_dev, sizeof(uint32_t) * 2 * (size_t)n_obs, cudaMemcpyDeviceToDevice, st));
+        if (C) CVB_CUDA(ctx, cudaMemcpyAsync(cons_out, cons_dev, sizeof(cvb_view_constraint) * C, cudaMemcpyDeviceToDevice, st));
+        R.counts.V = V; R.counts.n_features = nf; R.counts.L = L; R.counts.n_observations = n_obs; R.counts.C = C;
+        have = true;
+    } else {
+        // 2. add_view.  Its landmark count follows from the matches without a wait: L - merges + (N - matches)
+        uint32_t merges = 0;
+        {
+            hm.resize(M);
+            if (M) CVB_CUDA(ctx, cudaMemcpyAsync(hm.data(), mt, sizeof(cvb_register_match) * M, cudaMemcpyDeviceToHost, st));
+            CVB_CUDA(ctx, cvb_wait(ctx, st));
+            for (const cvb_register_match &m : hm) merges += m.landmark_b != CVB_REGISTER_NONE;
+        }
+        const uint32_t La = L - merges + (N - M);
+        if ((rc = add_view_enqueue(ctx, V, poses_dev, view_off_dev, view_lm_dev, bear_dev, desc_dev, col_dev, nf, L, lm_off_dev, obs_dev, n_obs,
+                                   &rres->pose, new_bear_dev, new_desc_dev, new_col_dev, N, mt, M, a.poses, a.vo, a.vl, a.bear, a.desc, a.col, a.lo,
+                                   a.obs, amap, cnt)))
+            return rc;
+        if (C) CVB_CUDA(ctx, cudaMemcpyAsync(a.cons, cons_dev, sizeof(cvb_view_constraint) * C, cudaMemcpyDeviceToDevice, st));
+        // 3. the new view's constraints and record_view_constraints' acceptance
+        const uint32_t q = V;
+        if ((rc = view_constraints_dev(ctx, ccfg, tri, V1, a.poses, a.vo, a.vl, a.bear, nf1, La, a.lo, a.obs, no1, &q, 1, a.cons + C, cres, nullptr)))
+            return rc;
+        CVB_CUDA(ctx, cudaMemcpyAsync(&R.con, cres, sizeof(cvb_view_constraints_result), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        const uint32_t Ca = C + R.con.n_constraints;
+        if (!R.con.accepted) {
+            // remove_view of the new view: the merges stay
+            R.status = CVB_INCORPORATE_REJECTED;
+            CVB_CUDA(ctx, cudaMemsetAsync(vs, CVB_RECON_VIEW_KEPT, V, st));
+            CVB_CUDA(ctx, cudaMemsetAsync(vs + V, CVB_RECON_VIEW_NO_EDGES, 1, st));
+            if (no1) {
+                k_inc_reject_states<<<cdiv(no1, 256), 256, 0, st>>>(no1, V, a.obs, os);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            if ((rc = apply_enqueue(ctx, V1, a.poses, a.vo, a.bear, a.desc, a.col, nf1, La, a.lo, a.obs, no1, a.cons, C, vs, os, poses_out,
+                                    view_off_out, view_lm_out, bear_out, desc_out, col_out, lm_off_out, obs_out, cons_out, avmap, almap,
+                                    cnt + 1)))
+                return rc;
+            have = edited = true;
+        } else {
+            // 4. optimize_reconstruction over the old constraints and the new ones, then its edits
+            if ((rc = optimize_reconstruction_dev(ctx, ocfg, tri, V1, a.poses, a.vo, a.vl, a.bear, nf1, La, a.lo, a.obs, no1, a.cons, Ca, ores,
+                                                  pout, vs, os)))
+                return rc;
+            CVB_CUDA(ctx, cudaMemcpyAsync(&R.recon, ores, sizeof(cvb_recon_result), cudaMemcpyDeviceToHost, st));
+            CVB_CUDA(ctx, cvb_wait(ctx, st));
+            if (R.recon.status == CVB_RECON_KEPT) {
+                R.status = CVB_INCORPORATE_KEPT;
+                if ((rc = apply_enqueue(ctx, V1, pout, a.vo, a.bear, a.desc, a.col, nf1, La, a.lo, a.obs, no1, a.cons, Ca, vs, os, poses_out,
+                                        view_off_out, view_lm_out, bear_out, desc_out, col_out, lm_off_out, obs_out, cons_out, avmap, almap,
+                                        cnt + 1)))
+                    return rc;
+                have = edited = true;
+            } else {
+                R.status = R.recon.status == CVB_RECON_REMOVED_CONSTRAINTS ? CVB_INCORPORATE_REMOVED_CONSTRAINTS
+                         : R.recon.status == CVB_RECON_REMOVED_FILTER      ? CVB_INCORPORATE_REMOVED_FILTER
+                                                                           : CVB_INCORPORATE_RECON_PANIC;
+            }
+        }
+    }
+    // the maps from the input to the output
+    if (!have) {
+        if (V) CVB_CUDA(ctx, cudaMemsetAsync(vmap, 0xff, sizeof(uint32_t) * V, st));
+        if (L) CVB_CUDA(ctx, cudaMemsetAsync(lmap, 0xff, sizeof(uint32_t) * L, st));
+    } else {
+        k_inc_compose<<<cdiv(V, 256), 256, 0, st>>>(V, nullptr, V1, edited ? avmap : nullptr, vmap);
+        CVB_LAUNCH_CHECK(ctx);
+        if (L) {
+            k_inc_compose<<<cdiv(L, 256), 256, 0, st>>>(L, edited ? amap : nullptr, L1, edited ? almap : nullptr, lmap);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+    }
+    if (edited) {
+        uint32_t nv = CVB_INCORPORATE_NONE;
+        CVB_CUDA(ctx, cudaMemcpyAsync(&R.counts, cnt + 1, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(&nv, avmap + V, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        R.new_view = nv;
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(res_dev, &R, sizeof(R), cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+namespace {
+
+// the host snapshot into the context's output workspace (as export_upload, with descriptors and colours), `extra` bytes after it
+int inc_upload(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc,
+               const uint8_t *col, uint32_t L, const uint32_t *lo, const uint32_t *obs, const cvb_view_constraint *cons, uint32_t C, size_t extra,
+               IncSnap &s, unsigned char *&b, size_t &end) {
+    const uint32_t nf = vo[V], no = lo[L];
+    size_t o[9];
+    end = inc_snap_layout(0, V, nf, L, no, C, desc != nullptr, col != nullptr, o);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = g->out.ensure(ctx, end + extra))) return rc;
+    b = (unsigned char *)g->out.p;
+    s = inc_snap_at(b, o, desc != nullptr, col != nullptr);
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(s.poses, poses, sizeof(cvb_pose) * V, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(s.vo, vo, sizeof(uint32_t) * ((size_t)V + 1), cudaMemcpyHostToDevice, st));
+    if (nf) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(s.vl, vl, sizeof(uint32_t) * (size_t)nf, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(s.bear, bear, sizeof(double) * 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+        if (desc) CVB_CUDA(ctx, cudaMemcpyAsync(s.desc, desc, 64 * (size_t)nf, cudaMemcpyHostToDevice, st));
+        if (col) CVB_CUDA(ctx, cudaMemcpyAsync(s.col, col, 3 * (size_t)nf, cudaMemcpyHostToDevice, st));
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(s.lo, lo, sizeof(uint32_t) * ((size_t)L + 1), cudaMemcpyHostToDevice, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(s.obs, obs, sizeof(uint32_t) * 2 * (size_t)no, cudaMemcpyHostToDevice, st));
+    if (C) CVB_CUDA(ctx, cudaMemcpyAsync(s.cons, cons, sizeof(cvb_view_constraint) * (size_t)C, cudaMemcpyHostToDevice, st));
+    return 0;
+}
+
+// an output snapshot of the given counts back to the host
+int inc_download(cvb_ctx *ctx, const IncSnap &s, const cvb_incorporate_counts &c, bool desc, bool col, cvb_pose *poses, uint32_t *vo,
+                 uint32_t *vl, double *bear, uint8_t *d, uint8_t *co, uint32_t *lo, uint32_t *obs, cvb_view_constraint *cons) {
+    cudaStream_t st = ctx->stream;
+    if (c.V) CVB_CUDA(ctx, cudaMemcpyAsync(poses, s.poses, sizeof(cvb_pose) * c.V, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(vo, s.vo, sizeof(uint32_t) * ((size_t)c.V + 1), cudaMemcpyDeviceToHost, st));
+    if (c.n_features) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(vl, s.vl, sizeof(uint32_t) * (size_t)c.n_features, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(bear, s.bear, sizeof(double) * 3 * (size_t)c.n_features, cudaMemcpyDeviceToHost, st));
+        if (desc) CVB_CUDA(ctx, cudaMemcpyAsync(d, s.desc, 64 * (size_t)c.n_features, cudaMemcpyDeviceToHost, st));
+        if (col) CVB_CUDA(ctx, cudaMemcpyAsync(co, s.col, 3 * (size_t)c.n_features, cudaMemcpyDeviceToHost, st));
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(lo, s.lo, sizeof(uint32_t) * ((size_t)c.L + 1), cudaMemcpyDeviceToHost, st));
+    if (c.n_observations) CVB_CUDA(ctx, cudaMemcpyAsync(obs, s.obs, sizeof(uint32_t) * 2 * (size_t)c.n_observations, cudaMemcpyDeviceToHost, st));
+    if (c.C && cons) CVB_CUDA(ctx, cudaMemcpyAsync(cons, s.cons, sizeof(cvb_view_constraint) * (size_t)c.C, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+}  // namespace
+
+int add_view(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc,
+             const uint8_t *col, uint32_t L, const uint32_t *lo, const uint32_t *obs, const cvb_pose *new_pose, const double *new_bear,
+             const uint8_t *new_desc, const uint8_t *new_col, uint32_t N, const cvb_register_match *matches, uint32_t M, cvb_pose *poses_out,
+             uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out,
+             uint32_t *lmap, cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!poses || !new_pose || !poses_out || !vo_out || !lo_out || !counts) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (incorporate_check(V, vo, vl, L, lo, obs, nullptr, 0, N, matches, M, nullptr, 0, nullptr, 0))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot or matches");
+    const uint32_t nf = vo[V], no = lo[L];
+    if ((nf && !bear) || (N && !new_bear) || (nf + N && (!vl_out || !bear_out)) || (no + N && !obs_out) || (L && !lmap))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!desc != !desc_out)) || (N && (!new_desc != !desc_out)) || (nf && (!col != !col_out)) || (N && (!new_col != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with the snapshot, the new frame and the output together");
+    const bool hd = desc_out != nullptr, hc = col_out != nullptr;
+    size_t x = 0, o[9];
+    const size_t i_np = x; x += con_align(sizeof(cvb_pose));
+    const size_t i_nb = x; x += con_align(sizeof(double) * 3 * std::max<size_t>(N, 1));
+    const size_t i_nd = x; x += con_align(64 * std::max<size_t>(N, 1));
+    const size_t i_nc = x; x += con_align(3 * std::max<size_t>(N, 1));
+    const size_t i_m = x; x += con_align(sizeof(cvb_register_match) * std::max<size_t>(M, 1));
+    const size_t i_map = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t i_cnt = x; x += con_align(sizeof(cvb_incorporate_counts));
+    x = inc_snap_layout(x, V + 1, nf + N, L + N, no + N, 0, hd, hc, o);
+    IncSnap s;
+    unsigned char *b;
+    size_t end;
+    int rc;
+    if ((rc = inc_upload(ctx, V, poses, vo, vl, bear, hd ? desc : nullptr, hc ? col : nullptr, L, lo, obs, nullptr, 0, x, s, b, end))) return rc;
+    unsigned char *e = b + end;
+    cudaStream_t st = ctx->stream;
+    CVB_CUDA(ctx, cudaMemcpyAsync(e + i_np, new_pose, sizeof(cvb_pose), cudaMemcpyHostToDevice, st));
+    if (N) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nb, new_bear, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, st));
+        if (hd) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nd, new_desc, 64 * (size_t)N, cudaMemcpyHostToDevice, st));
+        if (hc) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nc, new_col, 3 * (size_t)N, cudaMemcpyHostToDevice, st));
+    }
+    if (M) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_m, matches, sizeof(cvb_register_match) * M, cudaMemcpyHostToDevice, st));
+    IncSnap out = inc_snap_at(e, o, hd, hc);
+    if ((rc = add_view_dev(ctx, V, s.poses, s.vo, s.vl, s.bear, s.desc, s.col, nf, L, s.lo, s.obs, no, (const cvb_pose *)(e + i_np),
+                           (const double *)(e + i_nb), hd ? e + i_nd : nullptr, hc ? e + i_nc : nullptr, N, (const cvb_register_match *)(e + i_m), M,
+                           out.poses, out.vo, out.vl, out.bear, out.desc, out.col, out.lo, out.obs, (uint32_t *)(e + i_map),
+                           (cvb_incorporate_counts *)(e + i_cnt))))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(counts, e + i_cnt, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+    if (L) CVB_CUDA(ctx, cudaMemcpyAsync(lmap, e + i_map, sizeof(uint32_t) * L, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return inc_download(ctx, out, *counts, hd, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, nullptr);
+}
+
+int apply_optimization(cvb_ctx *ctx, uint32_t V, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear,
+                       const uint8_t *desc, const uint8_t *col, uint32_t L, const uint32_t *lo, const uint32_t *obs, const cvb_view_constraint *cons,
+                       uint32_t C, const uint8_t *vstate, const uint8_t *ostate, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out,
+                       double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out,
+                       uint32_t *vmap, uint32_t *lmap, cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!poses || !vstate || !poses_out || !vo_out || !lo_out || !counts || (V && !vmap) || (L && !lmap) || (C && !cons_out))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (incorporate_check(V, vo, vl, L, lo, obs, cons, C, 0, nullptr, 0, vstate, V, ostate, lo ? lo[L] : 0))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot, constraints or states");
+    const uint32_t nf = vo[V], no = lo[L];
+    if ((nf && (!bear || !vl_out || !bear_out)) || (no && !obs_out)) return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (nf && ((!desc != !desc_out) || (!col != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with the snapshot and the output together");
+    const bool hd = desc_out != nullptr, hc = col_out != nullptr;
+    size_t x = 0, o[9];
+    const size_t i_vs = x; x += con_align(std::max<size_t>(V, 1));
+    const size_t i_os = x; x += con_align(std::max<size_t>(no, 1));
+    const size_t i_vmap = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(V, 1));
+    const size_t i_lmap = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t i_cnt = x; x += con_align(sizeof(cvb_incorporate_counts));
+    x = inc_snap_layout(x, V, nf, L + no, no, C, hd, hc, o);
+    IncSnap s;
+    unsigned char *b;
+    size_t end;
+    int rc;
+    if ((rc = inc_upload(ctx, V, poses, vo, vl, bear, hd ? desc : nullptr, hc ? col : nullptr, L, lo, obs, cons, C, x, s, b, end))) return rc;
+    unsigned char *e = b + end;
+    cudaStream_t st = ctx->stream;
+    if (V) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_vs, vstate, V, cudaMemcpyHostToDevice, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_os, ostate, no, cudaMemcpyHostToDevice, st));
+    IncSnap out = inc_snap_at(e, o, hd, hc);
+    if ((rc = apply_optimization_dev(ctx, V, s.poses, s.vo, s.vl, s.bear, s.desc, s.col, nf, L, s.lo, s.obs, no, s.cons, C, e + i_vs, e + i_os,
+                                     out.poses, out.vo, out.vl, out.bear, out.desc, out.col, out.lo, out.obs, out.cons, (uint32_t *)(e + i_vmap),
+                                     (uint32_t *)(e + i_lmap), (cvb_incorporate_counts *)(e + i_cnt))))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(counts, e + i_cnt, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+    if (V) CVB_CUDA(ctx, cudaMemcpyAsync(vmap, e + i_vmap, sizeof(uint32_t) * V, cudaMemcpyDeviceToHost, st));
+    if (L) CVB_CUDA(ctx, cudaMemcpyAsync(lmap, e + i_lmap, sizeof(uint32_t) * L, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return inc_download(ctx, out, *counts, hd, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
+}
+
+int incorporate_frame(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_constraints_cfg *ccfg, const cvb_recon_cfg *ocfg,
+                      const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng, uint32_t V, const cvb_pose *poses, const uint32_t *vo,
+                      const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t L, const uint32_t *lo,
+                      const uint32_t *obs, const cvb_view_constraint *cons, uint32_t C, const uint8_t *new_desc, const double *new_bear,
+                      const uint8_t *new_col, uint32_t N, const uint32_t *view_matches, uint32_t H, cvb_pose *poses_out, uint32_t *vo_out,
+                      uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out,
+                      cvb_view_constraint *cons_out, uint32_t *vmap, uint32_t *lmap, cvb_register_match *matches, cvb_incorporate_result *res) {
+    if (!ctx) return CVB_EINVAL;
+    if (!rcfg || !ccfg || !ocfg || !tri || !arrsac || !rng || !poses || !res || !poses_out || !vo_out || !lo_out || !cons_out ||
+        (V && !vmap) || (L && !lmap) || (N && (!new_desc || !new_bear)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (incorporate_check(V, vo, vl, L, lo, obs, cons, C, 0, nullptr, 0, nullptr, 0, nullptr, 0) ||
+        register_check(V, vo, vl, L, lo, obs, view_matches, H))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshot, constraints or view matches");
+    const uint32_t nf = vo[V], no = lo[L];
+    if ((nf && (!bear || !desc)) || (nf + N && (!vl_out || !bear_out || !desc_out)) || (no + N && !obs_out))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!col != !col_out)) || (N && (!new_col != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "colours go with the snapshot, the new frame and the output together");
+    const bool hc = col_out != nullptr;
+    const uint32_t maxc = ccfg->optimization_maximum_three_view_constraints;
+    size_t x = 0, o[9];
+    const size_t i_nd = x; x += con_align(64 * std::max<size_t>(N, 1));
+    const size_t i_nb = x; x += con_align(sizeof(double) * 3 * std::max<size_t>(N, 1));
+    const size_t i_nc = x; x += con_align(3 * std::max<size_t>(N, 1));
+    const size_t i_m = x; x += con_align(sizeof(cvb_register_match) * std::max<size_t>(N, 1));
+    const size_t i_vmap = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(V, 1));
+    const size_t i_lmap = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t i_res = x; x += con_align(sizeof(cvb_incorporate_result));
+    x = inc_snap_layout(x, V + 1, nf + N, L + N + no + N, no + N, C + maxc, true, hc, o);
+    IncSnap s;
+    unsigned char *b;
+    size_t end;
+    int rc;
+    if ((rc = inc_upload(ctx, V, poses, vo, vl, bear, desc, hc ? col : nullptr, L, lo, obs, cons, C, x, s, b, end))) return rc;
+    unsigned char *e = b + end;
+    cudaStream_t st = ctx->stream;
+    if (N) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nd, new_desc, 64 * (size_t)N, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nb, new_bear, sizeof(double) * 3 * (size_t)N, cudaMemcpyHostToDevice, st));
+        if (hc) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_nc, new_col, 3 * (size_t)N, cudaMemcpyHostToDevice, st));
+    }
+    IncSnap out = inc_snap_at(e, o, true, hc);
+    cvb_incorporate_result *rd = (cvb_incorporate_result *)(e + i_res);
+    if ((rc = incorporate_frame_dev(ctx, rcfg, ccfg, ocfg, tri, arrsac, rng, V, s.poses, s.vo, s.vl, s.bear, s.desc, s.col, nf, L, s.lo, s.obs, no,
+                                    s.cons, C, e + i_nd, (const double *)(e + i_nb), hc ? e + i_nc : nullptr, N, view_matches, H, out.poses, out.vo,
+                                    out.vl, out.bear, out.desc, out.col, out.lo, out.obs, out.cons, (uint32_t *)(e + i_vmap), (uint32_t *)(e + i_lmap),
+                                    (cvb_register_match *)(e + i_m), rd)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, rd, sizeof(cvb_incorporate_result), cudaMemcpyDeviceToHost, st));
+    if (V) CVB_CUDA(ctx, cudaMemcpyAsync(vmap, e + i_vmap, sizeof(uint32_t) * V, cudaMemcpyDeviceToHost, st));
+    if (L) CVB_CUDA(ctx, cudaMemcpyAsync(lmap, e + i_lmap, sizeof(uint32_t) * L, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    const uint32_t M = res->reg.status == CVB_REGISTER_OK ? res->reg.n_matches : 0;
+    if (matches && M) CVB_CUDA(ctx, cudaMemcpyAsync(matches, e + i_m, sizeof(cvb_register_match) * M, cudaMemcpyDeviceToHost, st));
+    const bool have = res->status == CVB_INCORPORATE_KEPT || res->status == CVB_INCORPORATE_REJECTED || res->status == CVB_INCORPORATE_NOT_REGISTERED;
+    if (!have) {
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        return 0;
+    }
+    return inc_download(ctx, out, res->counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
 }
 
 extern "C" {
