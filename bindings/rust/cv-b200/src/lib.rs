@@ -222,3 +222,6 @@ pub mod register;
 
 // ---- INTEGRATION.md section 2q (include/cvb200_incorporate.h) ----
 pub mod incorporate;
+
+// ---- INTEGRATION.md section 2r (include/cvb200_merge.h) ----
+pub mod merge;

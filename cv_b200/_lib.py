@@ -4,7 +4,8 @@ cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (i
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
 (include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h), cv_b200/libcvb200_reconstruction.so
 (include/cvb200_reconstruction.h), cv_b200/libcvb200_export.so (include/cvb200_export.h) and
-cv_b200/libcvb200_register.so (include/cvb200_register.h) and cv_b200/libcvb200_incorporate.so (include/cvb200_incorporate.h)."""
+cv_b200/libcvb200_register.so (include/cvb200_register.h), cv_b200/libcvb200_incorporate.so (include/cvb200_incorporate.h) and
+cv_b200/libcvb200_merge.so (include/cvb200_merge.h)."""
 import ctypes as C
 import os
 
@@ -146,6 +147,10 @@ REGISTER_ABI_SYMBOLS = ["cvb_register_cfg_default", "cvb_register_check", "cvb_r
 # tests/test_abi_incorporate.py
 INCORPORATE_ABI_SYMBOLS = ["cvb_incorporate_check", "cvb_add_view_dev", "cvb_add_view", "cvb_apply_optimization_dev", "cvb_apply_optimization",
                            "cvb_incorporate_frame_dev", "cvb_incorporate_frame"]
+# every symbol include/cvb200_merge.h declares (cv-sfm's reconstruction merging), exported by libcvb200_merge.so; checked by
+# tests/test_abi_merge.py
+MERGE_ABI_SYMBOLS = ["cvb_merge_check", "cvb_incorporate_reconstruction_dev", "cvb_incorporate_reconstruction", "cvb_merge_reconstructions_dev",
+                     "cvb_merge_reconstructions"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -517,6 +522,36 @@ def load_incorporate_library():
         L.cvb_incorporate_frame.argtypes = [vp] * 7 + [u32] + [vp] * 6 + [u32, vp, vp, vp, u32, vp, vp, vp, u32, vp, u32] + [vp] * 13
         _INCORPORATE_LIB = L
     return _INCORPORATE_LIB
+
+
+_MERGE_LIB = None
+
+
+def merge_lib_path():
+    return os.path.join(_HERE, "libcvb200_merge.so")
+
+
+def load_merge_library():
+    """Loads libcvb200_merge.so, the module of include/cvb200_merge.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _MERGE_LIB
+    if _MERGE_LIB is None:
+        load_library()
+        p = merge_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32, i32 = C.c_void_p, C.c_uint32, C.c_int
+        L.cvb_merge_check.argtypes = [u32, vp, vp, u32, vp, vp, vp, u32, u32, vp, vp, u32, vp, vp, u32, vp, i32, i32]
+        L.cvb_incorporate_reconstruction_dev.argtypes = ([vp] * 3 + [u32] + [vp] * 6 + [u32, u32, vp, vp, u32, vp, u32, u32] + [vp] * 6 +
+                                                         [u32, u32, vp, vp, u32, u32, vp, vp] + [vp] * 13)
+        L.cvb_incorporate_reconstruction.argtypes = ([vp] * 3 + [u32] + [vp] * 6 + [u32, vp, vp, vp, u32, u32] + [vp] * 6 +
+                                                     [u32, vp, vp, u32, vp, vp] + [vp] * 13)
+        L.cvb_merge_reconstructions_dev.argtypes = ([vp] * 7 + [u32] + [vp] * 6 + [u32, u32, vp, vp, u32, vp, u32, u32] + [vp] * 6 +
+                                                    [u32, u32, vp, vp, u32, u32, vp, u32] + [vp] * 15)
+        L.cvb_merge_reconstructions.argtypes = ([vp] * 7 + [u32] + [vp] * 6 + [u32, vp, vp, vp, u32, u32] + [vp] * 6 +
+                                                [u32, vp, vp, u32, vp, u32] + [vp] * 15)
+        _MERGE_LIB = L
+    return _MERGE_LIB
 
 
 class Context:

@@ -66,8 +66,8 @@ def generate_view_constraints(ctx, poses, view_offsets, view_landmarks, bearings
 
     Returns dict(constraints: per query a CONSTRAINT_DTYPE array in the reference's evaluation order, results: RESULT_DTYPE [Q]
     (n_constraints, accepted = record_view_constraints' return), stats: STATS_DTYPE [Q] or None).  A call over every view is
-    regenerate_reconstruction's constraint pass; incorporate_reconstruction removes views between its calls, so call it one view at a time
-    there.  Unpinned, as the reference leaves these orders undefined: coviews ascending, stable sorts, no shuffle of the landmarks,
+    regenerate_reconstruction's constraint pass; incorporate_reconstruction removes views between its calls, which
+    cv_b200.incorporate_reconstruction does by repeating the call after each refusal.  Unpinned, as the reference leaves these orders undefined: coviews ascending, stable sorts, no shuffle of the landmarks,
     observations in the given order."""
     from .triangulation import LinearEigenTriangulator
     settings = settings if settings is not None else ConstraintSettings()

@@ -25,6 +25,7 @@
 #include "../../include/cvb200_export.h"
 #include "../../include/cvb200_register.h"
 #include "../../include/cvb200_incorporate.h"
+#include "../../include/cvb200_merge.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1581,6 +1582,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 #include "export_dev.cuh"
 #include "register_dev.cuh"
 #include "incorporate_dev.cuh"
+#include "merge_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1744,12 +1746,13 @@ struct GeomWorkspace {
     DevBuf exp;                     // the export's workspace (export_dev.cuh's drivers)
     DevBuf reg;                     // frame registration's workspace (register_frame_dev)
     DevBuf inc, incs;               // frame incorporation's snapshot after add_view and the two edits' scratch (incorporate_frame_dev)
+    DevBuf mrg, mrgs;               // merging's snapshot after add_view, and the move's snapshots and scratch (merge_dev.cuh's drivers)
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2, &g->rec, &g->exp, &g->reg, &g->inc, &g->incs};
+                      &g->con2, &g->rec, &g->exp, &g->reg, &g->inc, &g->incs, &g->mrg, &g->mrgs};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -4526,6 +4529,614 @@ int incorporate_frame(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_cons
         CVB_CUDA(ctx, cvb_wait(ctx, st));
         return 0;
     }
+    return inc_download(ctx, out, res->counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
+}
+
+// ---- cv-sfm's reconstruction merging (C names in merge_abi.cu, include/cvb200_merge.h; kernels in merge_dev.cuh) ------------------------
+int merge_check(uint32_t V, const uint32_t *vo, const uint32_t *vl, uint32_t L, const uint32_t *lo, const uint32_t *obs,
+                const cvb_view_constraint *cons, uint32_t C, uint32_t VS, const uint32_t *vo_s, const uint32_t *vl_s, uint32_t LS,
+                const uint32_t *lo_s, const uint32_t *obs_s, uint32_t view_s, const uint32_t *lmap, int has_col, int has_col_s) {
+    if (incorporate_check(V, vo, vl, L, lo, obs, cons, C, 0, nullptr, 0, nullptr, 0, nullptr, 0)) return CVB_EINVAL;
+    if (incorporate_check(VS, vo_s, vl_s, LS, lo_s, obs_s, nullptr, 0, 0, nullptr, 0, nullptr, 0, nullptr, 0)) return CVB_EINVAL;
+    if (!has_col != !has_col_s) return CVB_EINVAL;
+    if (view_s >= VS && !(view_s == CVB_MERGE_NONE && lmap)) return CVB_EINVAL;
+    if (lmap) {
+        std::vector<uint8_t> used(L, 0);
+        for (uint32_t l = 0; l < LS; l++) {
+            if (lmap[l] == CVB_MERGE_NONE) continue;
+            if (lmap[l] >= L || used[lmap[l]]) return CVB_EINVAL;   // HashMap::insert would overwrite an observation of one view
+            used[lmap[l]] = 1;
+        }
+    }
+    return 0;
+}
+
+namespace {
+
+// the move edit and the speculative constraint loop of incorporate_reconstruction on device arrays (D: V views, C constraints; S's view
+// CSR and landmark CSR).  Leaves the final snapshot in the context's merge scratch (*fin, counts in R.counts), the source landmark map
+// (device, LS entries) in *tgt_fin, and on the host the source view map and each moved view's constraint result.
+int move_and_constrain(cvb_ctx *ctx, const cvb_constraints_cfg *ccfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                       const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t nf, uint32_t L,
+                       const uint32_t *lo, const uint32_t *obs, uint32_t n_obs, const cvb_view_constraint *cons, uint32_t C, uint32_t VS,
+                       const cvb_pose *poses_s, const uint32_t *vo_s, const uint32_t *vl_s, const double *bear_s, const uint8_t *desc_s,
+                       const uint8_t *col_s, uint32_t nf_s, uint32_t LS, const uint32_t *lo_s, const uint32_t *obs_s, uint32_t n_obs_s,
+                       uint32_t skip, uint32_t nf_skip, const cvb_pose *wt, const uint32_t *lmap_in, IncSnap &fin, const uint32_t *&tgt_fin,
+                       std::vector<uint32_t> &svmap, std::vector<cvb_view_constraints_result> &cres, cvb_move_result &R) {
+    cudaStream_t st = ctx->stream;
+    const bool hd = desc != nullptr, hc = col != nullptr;
+    const uint32_t Q = VS - (skip < VS ? 1u : 0u), maxc = ccfg->optimization_maximum_three_view_constraints;
+    const uint32_t VA = V + Q, nfA = nf + nf_s, LA = L + nf_s, noA = n_obs + nf_s, CA = C + Q * maxc, n = L + nf_s;
+    size_t oa[9], ob[9], off = 0;
+    off = inc_snap_layout(off, VA, nfA, LA, noA, CA, hd, hc, oa);
+    off = inc_snap_layout(off, VA, nfA, LA, noA, CA, hd, hc, ob);
+    const size_t o_conq = off; off += con_align(sizeof(cvb_view_constraint) * std::max<size_t>((size_t)Q * maxc, 1));
+    const size_t o_resq = off; off += con_align(sizeof(cvb_view_constraints_result) * std::max<size_t>(Q, 1));
+    const size_t o_cnt = off; off += con_align(sizeof(uint2) * std::max<size_t>(n, 1));
+    const size_t o_tiles = off; off += con_align(sizeof(uint2) * std::max<size_t>(cdiv(n, INC_TILE), 1));
+    const size_t o_tot = off; off += con_align(sizeof(uint2));
+    const size_t o_app = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t o_first = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t o_tgt0 = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t o_tgt1 = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t o_vmap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(VA, 1));
+    const size_t o_lmap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LA, 1));
+    const size_t o_vs = off; off += con_align(std::max<size_t>(VA, 1));
+    const size_t o_os = off; off += con_align(std::max<size_t>(noA, 1));
+    const size_t o_counts = off; off += con_align(sizeof(cvb_incorporate_counts));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->mrgs.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->mrgs.p;
+    IncSnap A = inc_snap_at(b, oa, hd, hc), B = inc_snap_at(b, ob, hd, hc);
+    cvb_view_constraint *conq = (cvb_view_constraint *)(b + o_conq);
+    cvb_view_constraints_result *resq = (cvb_view_constraints_result *)(b + o_resq);
+    uint2 *cnt = (uint2 *)(b + o_cnt), *tiles = (uint2 *)(b + o_tiles), *total = (uint2 *)(b + o_tot);
+    uint32_t *app = (uint32_t *)(b + o_app), *first = (uint32_t *)(b + o_first), *tgt[2] = {(uint32_t *)(b + o_tgt0), (uint32_t *)(b + o_tgt1)};
+    uint32_t *vmap_ap = (uint32_t *)(b + o_vmap), *lmap_ap = (uint32_t *)(b + o_lmap);
+    uint8_t *vs = b + o_vs, *os = b + o_os;
+    cvb_incorporate_counts *dcnt = (cvb_incorporate_counts *)(b + o_counts);
+    // 1. the move
+    CVB_PROF(ctx, "k_mg", 0);
+    CVB_CUDA(ctx, cudaMemsetAsync(cnt, 0, sizeof(uint2) * std::max<size_t>(n, 1), st));
+    if (L) CVB_CUDA(ctx, cudaMemsetAsync(app, 0, sizeof(uint32_t) * L, st));
+    if (LS) {
+        k_mg_landmark_counts<<<cdiv(LS, 256), 256, 0, st>>>(LS, n_obs_s, VS, nf_s, skip, L, lo_s, obs_s, vo_s, lmap_in, app, cnt, first);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (L) {
+        k_mg_dest_counts<<<cdiv(L, 256), 256, 0, st>>>(L, n_obs, lo, app, cnt);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if ((rc = inc_scan(ctx, n, cnt, tiles, total))) return rc;
+    if (L) {
+        k_mg_dest_place<<<cdiv(L, 256), 256, 0, st>>>(L, n_obs, lo, obs, cnt, noA, A.lo, A.obs);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    if (LS) {
+        k_mg_landmark_place<<<cdiv(LS, 256), 256, 0, st>>>(LS, n_obs_s, VS, nf_s, skip, V, L, n_obs, lo_s, obs_s, vo_s, lmap_in, lo, cnt, first, LA,
+                                                           noA, A.lo, A.obs, tgt[0]);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(A.poses, poses, sizeof(cvb_pose) * V, cudaMemcpyDeviceToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(A.vo, vo, sizeof(uint32_t) * ((size_t)V + 1), cudaMemcpyDeviceToDevice, st));
+    if (nf) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(A.vl, vl, sizeof(uint32_t) * nf, cudaMemcpyDeviceToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(A.bear, bear, sizeof(double) * 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+        if (hd) CVB_CUDA(ctx, cudaMemcpyAsync(A.desc, desc, 64 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+        if (hc) CVB_CUDA(ctx, cudaMemcpyAsync(A.col, col, 3 * (size_t)nf, cudaMemcpyDeviceToDevice, st));
+    }
+    if (C) CVB_CUDA(ctx, cudaMemcpyAsync(A.cons, cons, sizeof(cvb_view_constraint) * C, cudaMemcpyDeviceToDevice, st));
+    if (VS) {
+        k_mg_views<<<cdiv(VS, 128), 128, 0, st>>>(VS, skip, V, nf, nf_s, poses_s, vo_s, wt, A.poses, A.vo);
+        CVB_LAUNCH_CHECK(ctx);
+        k_mg_feature_rows<<<cdiv(VS * 32, 256), 256, 0, st>>>(VS, skip, nf, nf_s, LS, vo_s, vl_s, bear_s, (const uint4 *)desc_s, col_s, tgt[0], nfA,
+                                                              A.vl, A.bear, (uint4 *)A.desc, A.col);
+        CVB_LAUNCH_CHECK(ctx);
+    }
+    const uint32_t nf_moved = nf_s >= nf_skip ? nf_s - nf_skip : 0;
+    k_mg_finish<<<1, 1, 0, st>>>(V, Q, nf + nf_moved, total, LA, noA, A.vo, A.lo, dcnt);
+    CVB_LAUNCH_CHECK(ctx);
+    cvb_incorporate_counts c;
+    CVB_CUDA(ctx, cudaMemcpyAsync(&c, dcnt, sizeof(c), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    memset(&R, 0, sizeof(R));
+    R.moved_views = Q;
+    R.created_landmarks = c.L - std::min(c.L, L);
+    // 2. the constraint loop: one call over every undecided moved view; the results up to the first refusal are final
+    std::vector<uint32_t> cur(Q), sv(Q);   // each moved view's current index and its S view
+    for (uint32_t v = 0, q = 0; v < VS; v++)
+        if (v != skip) { sv[q] = v; cur[q] = V + q; q++; }
+    cres.assign(VS, cvb_view_constraints_result{0, 0});
+    std::vector<uint8_t> refused(Q, 0);
+    std::vector<cvb_view_constraints_result> hres(std::max<uint32_t>(Q, 1));
+    std::vector<uint32_t> queries;
+    uint32_t Cc = C, start = 0, t = 0;
+    IncSnap *curS = &A, *nxtS = &B;
+    while (start < Q) {
+        queries.assign(cur.begin() + start, cur.end());
+        const uint32_t nq = Q - start;
+        if ((rc = view_constraints_dev(ctx, ccfg, tri, c.V, curS->poses, curS->vo, curS->vl, curS->bear, c.n_features, c.L, curS->lo, curS->obs,
+                                       c.n_observations, queries.data(), nq, conq, resq, nullptr)))
+            return rc;
+        R.constraint_calls++;
+        CVB_CUDA(ctx, cudaMemcpyAsync(hres.data(), resq, sizeof(cvb_view_constraints_result) * nq, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        uint32_t j = start;
+        for (; j < Q; j++) {
+            const cvb_view_constraints_result &r = hres[j - start];
+            cres[sv[j]] = r;
+            if (!r.accepted) break;
+            const uint32_t k = std::min(r.n_constraints, maxc);
+            if (k) CVB_CUDA(ctx, cudaMemcpyAsync(curS->cons + Cc, conq + (size_t)(j - start) * maxc, sizeof(cvb_view_constraint) * k,
+                                                 cudaMemcpyDeviceToDevice, st));
+            Cc += k;
+        }
+        if (j == Q) break;
+        // remove_view of the refused view j: its observations DROPPED, every other KEPT
+        refused[j] = 1;
+        R.refused_views++;
+        CVB_CUDA(ctx, cudaMemsetAsync(vs, CVB_RECON_VIEW_KEPT, c.V, st));
+        CVB_CUDA(ctx, cudaMemsetAsync(vs + cur[j], CVB_RECON_VIEW_NO_EDGES, 1, st));
+        if (c.n_observations) {
+            k_inc_reject_states<<<cdiv(c.n_observations, 256), 256, 0, st>>>(c.n_observations, cur[j], curS->obs, os);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        if ((rc = apply_enqueue(ctx, c.V, curS->poses, curS->vo, curS->bear, curS->desc, curS->col, c.n_features, c.L, curS->lo, curS->obs,
+                                c.n_observations, curS->cons, Cc, vs, os, nxtS->poses, nxtS->vo, nxtS->vl, nxtS->bear, nxtS->desc, nxtS->col,
+                                nxtS->lo, nxtS->obs, nxtS->cons, vmap_ap, lmap_ap, dcnt)))
+            return rc;
+        if (LS) {
+            k_inc_compose<<<cdiv(LS, 256), 256, 0, st>>>(LS, tgt[t], c.L, lmap_ap, tgt[t ^ 1]);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+        t ^= 1;
+        CVB_CUDA(ctx, cudaMemcpyAsync(&c, dcnt, sizeof(c), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        Cc = c.C;
+        for (uint32_t k = j + 1; k < Q; k++) cur[k]--;
+        std::swap(curS, nxtS);
+        start = j + 1;
+    }
+    c.C = Cc;
+    c.merges = 0;
+    R.counts = c;
+    svmap.assign(VS, CVB_MERGE_NONE);
+    for (uint32_t q = 0; q < Q; q++)
+        if (!refused[q]) svmap[sv[q]] = cur[q];
+    fin = *curS;
+    tgt_fin = tgt[t];
+    return 0;
+}
+
+// a snapshot of the given counts copied between device arrays
+int inc_copy(cvb_ctx *ctx, const IncSnap &s, const cvb_incorporate_counts &c, cvb_pose *poses, uint32_t *vo, uint32_t *vl, double *bear,
+             uint8_t *d, uint8_t *co, uint32_t *lo, uint32_t *obs, cvb_view_constraint *cons) {
+    cudaStream_t st = ctx->stream;
+    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
+    if (c.V) CVB_CUDA(ctx, cudaMemcpyAsync(poses, s.poses, sizeof(cvb_pose) * c.V, k, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(vo, s.vo, sizeof(uint32_t) * ((size_t)c.V + 1), k, st));
+    if (c.n_features) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(vl, s.vl, sizeof(uint32_t) * (size_t)c.n_features, k, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(bear, s.bear, sizeof(double) * 3 * (size_t)c.n_features, k, st));
+        if (d && s.desc) CVB_CUDA(ctx, cudaMemcpyAsync(d, s.desc, 64 * (size_t)c.n_features, k, st));
+        if (co && s.col) CVB_CUDA(ctx, cudaMemcpyAsync(co, s.col, 3 * (size_t)c.n_features, k, st));
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(lo, s.lo, sizeof(uint32_t) * ((size_t)c.L + 1), k, st));
+    if (c.n_observations) CVB_CUDA(ctx, cudaMemcpyAsync(obs, s.obs, sizeof(uint32_t) * 2 * (size_t)c.n_observations, k, st));
+    if (c.C) CVB_CUDA(ctx, cudaMemcpyAsync(cons, s.cons, sizeof(cvb_view_constraint) * (size_t)c.C, k, st));
+    return 0;
+}
+
+// two entries of a device offset array, read back
+int mg_row(cvb_ctx *ctx, const uint32_t *off_dev, uint32_t i, uint32_t n, uint32_t &r0, uint32_t &r1) {
+    uint32_t *h = (uint32_t *)cvb_pinned(ctx, 2 * sizeof(uint32_t));
+    if (!h) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(h, off_dev + i, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    r0 = std::min(h[0], n);
+    r1 = std::min(std::max(h[1], r0), n);
+    return 0;
+}
+
+// the refusals every device entry shares
+int mg_args(cvb_ctx *ctx, const cvb_constraints_cfg *ccfg, const cvb_triangulator *tri, uint32_t V) {
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: merging takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (ccfg->optimization_maximum_landmarks > CVB_CONSTRAINTS_MAX_LANDMARKS)
+        return cvb_set_error(ctx, CVB_EUNSUPPORTED, "optimization_maximum_landmarks %u > %u", ccfg->optimization_maximum_landmarks,
+                             CVB_CONSTRAINTS_MAX_LANDMARKS);
+    if (V == 0) return cvb_set_error(ctx, CVB_EINVAL, "no views");
+    return 0;
+}
+
+}  // namespace
+
+int incorporate_reconstruction_dev(cvb_ctx *ctx, const cvb_constraints_cfg *ccfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                                   const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t nf,
+                                   uint32_t L, const uint32_t *lo, const uint32_t *obs, uint32_t n_obs, const cvb_view_constraint *cons, uint32_t C,
+                                   uint32_t VS, const cvb_pose *poses_s, const uint32_t *vo_s, const uint32_t *vl_s, const double *bear_s,
+                                   const uint8_t *desc_s, const uint8_t *col_s, uint32_t nf_s, uint32_t LS, const uint32_t *lo_s,
+                                   const uint32_t *obs_s, uint32_t n_obs_s, uint32_t skip, const cvb_pose *wt, const uint32_t *lmap_in,
+                                   cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out,
+                                   uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, uint32_t *svmap_dev, uint32_t *slmap_dev,
+                                   cvb_view_constraints_result *cres_dev, cvb_move_result *res_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!ccfg || !tri || !poses || !vo || !lo || !poses_s || !vo_s || !lo_s || !wt || !poses_out || !vo_out || !lo_out || !res_dev ||
+        (nf && (!vl || !bear)) || (n_obs && !obs) || (C && !cons) || (nf_s && (!vl_s || !bear_s)) || (n_obs_s && !obs_s) ||
+        (LS && (!lmap_in || !slmap_dev)) || (VS && (!svmap_dev || !cres_dev)) || (nf + nf_s && (!vl_out || !bear_out)) ||
+        (n_obs + nf_s && !obs_out) || !cons_out)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!desc != !desc_out)) || (nf_s && (!desc_s != !desc_out)) || (nf && (!col != !col_out)) || (nf_s && (!col_s != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with both snapshots and the output together");
+    if (skip != CVB_MERGE_NONE && skip >= VS) return cvb_set_error(ctx, CVB_EINVAL, "skip_view %u >= V_S %u", skip, VS);
+    int rc;
+    if ((rc = mg_args(ctx, ccfg, tri, V))) return rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = inc_sizes(ctx, V, vo, nf, L, lo, n_obs))) return rc;
+    if ((rc = inc_sizes(ctx, VS, vo_s, nf_s, LS, lo_s, n_obs_s))) return rc;
+    uint32_t r0 = 0, r1 = 0;
+    if (skip < VS && (rc = mg_row(ctx, vo_s, skip, nf_s, r0, r1))) return rc;
+    IncSnap fin;
+    const uint32_t *tgt;
+    std::vector<uint32_t> svmap;
+    std::vector<cvb_view_constraints_result> cres;
+    cvb_move_result R;
+    if ((rc = move_and_constrain(ctx, ccfg, tri, V, poses, vo, vl, bear, desc_out ? desc : nullptr, col_out ? col : nullptr, nf, L, lo, obs, n_obs,
+                                 cons, C, VS, poses_s, vo_s, vl_s, bear_s, desc_out ? desc_s : nullptr, col_out ? col_s : nullptr, nf_s, LS, lo_s,
+                                 obs_s, n_obs_s, skip, r1 - r0, wt, lmap_in, fin, tgt, svmap, cres, R)))
+        return rc;
+    cudaStream_t st = ctx->stream;
+    if ((rc = inc_copy(ctx, fin, R.counts, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out))) return rc;
+    if (VS) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(svmap_dev, svmap.data(), sizeof(uint32_t) * VS, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(cres_dev, cres.data(), sizeof(cvb_view_constraints_result) * VS, cudaMemcpyHostToDevice, st));
+    }
+    if (LS) CVB_CUDA(ctx, cudaMemcpyAsync(slmap_dev, tgt, sizeof(uint32_t) * LS, cudaMemcpyDeviceToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(res_dev, &R, sizeof(R), cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int merge_reconstructions_dev(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_constraints_cfg *ccfg, const cvb_recon_cfg *ocfg,
+                              const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng, uint32_t V, const cvb_pose *poses,
+                              const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t nf,
+                              uint32_t L, const uint32_t *lo, const uint32_t *obs, uint32_t n_obs, const cvb_view_constraint *cons, uint32_t C,
+                              uint32_t VS, const cvb_pose *poses_s, const uint32_t *vo_s, const uint32_t *vl_s, const double *bear_s,
+                              const uint8_t *desc_s, const uint8_t *col_s, uint32_t nf_s, uint32_t LS, const uint32_t *lo_s, const uint32_t *obs_s,
+                              uint32_t n_obs_s, uint32_t s_view, const uint32_t *view_matches, uint32_t H, cvb_pose *poses_out, uint32_t *vo_out,
+                              uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out,
+                              cvb_view_constraint *cons_out, uint32_t *dvmap, uint32_t *dlmap, uint32_t *svmap_dev, uint32_t *slmap_dev,
+                              cvb_view_constraints_result *cres_dev, cvb_merge_result *res_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!rcfg || !ccfg || !ocfg || !tri || !arrsac || !rng || !poses || !vo || !lo || !poses_s || !vo_s || !lo_s || !poses_out || !vo_out ||
+        !lo_out || !res_dev || !cons_out || (H && !view_matches) || (nf && (!vl || !bear || !desc)) || (n_obs && !obs) || (C && !cons) ||
+        (nf_s && (!vl_s || !bear_s || !desc_s)) || (n_obs_s && !obs_s) || (nf + nf_s && (!vl_out || !bear_out || !desc_out)) ||
+        (n_obs + nf_s && !obs_out) || !dvmap || (L && !dlmap) || (VS && (!svmap_dev || !cres_dev)) || (LS && !slmap_dev))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!col != !col_out)) || (nf_s && (!col_s != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "colours go with both snapshots and the output together");
+    if (s_view >= VS) return cvb_set_error(ctx, CVB_EINVAL, "s_view %u >= V_S %u", s_view, VS);
+    int rc;
+    if ((rc = mg_args(ctx, ccfg, tri, V))) return rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = inc_sizes(ctx, V, vo, nf, L, lo, n_obs))) return rc;
+    if ((rc = inc_sizes(ctx, VS, vo_s, nf_s, LS, lo_s, n_obs_s))) return rc;
+    uint32_t r0, r1;
+    if ((rc = mg_row(ctx, vo_s, s_view, nf_s, r0, r1))) return rc;
+    const uint32_t N = r1 - r0;
+    cudaStream_t st = ctx->stream;
+    const bool hc = col_out != nullptr;
+    const uint32_t maxc = ccfg->optimization_maximum_three_view_constraints;
+    const uint32_t V1 = V + 1, nf1 = nf + N, L1 = L + N, no1 = n_obs + N, C1 = C + maxc;
+    const uint32_t VF = V + VS, LF = L + N + nf_s;   // the largest merged snapshot: views, landmarks
+    size_t o[9], off = 0;
+    const size_t o_rres = off; off += con_align(sizeof(cvb_register_result));
+    const size_t o_rst = off; off += con_align(sizeof(cvb_register_stats));
+    const size_t o_m = off; off += con_align(sizeof(cvb_register_match) * std::max<size_t>(N, 1));
+    const size_t o_cres = off; off += con_align(sizeof(cvb_view_constraints_result));
+    const size_t o_ores = off; off += con_align(sizeof(cvb_recon_result));
+    const size_t o_cnt = off; off += con_align(sizeof(cvb_incorporate_counts));
+    const size_t o_wt = off; off += con_align(sizeof(cvb_pose));
+    const size_t o_pout = off; off += con_align(sizeof(cvb_pose) * VF);
+    const size_t o_vs = off; off += con_align(VF);
+    const size_t o_os = off; off += con_align(std::max<size_t>((size_t)n_obs + N + nf_s, 1));
+    const size_t o_amap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t o_ltl = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t o_svm = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(VS, 1));
+    const size_t o_vmap = off; off += con_align(sizeof(uint32_t) * VF);
+    const size_t o_lmap = off; off += con_align(sizeof(uint32_t) * std::max<size_t>(LF, 1));
+    off = inc_snap_layout(off, V1, nf1, L1, no1, C1, true, hc, o);
+    GeomWorkspace *g = gws(ctx);
+    if ((rc = g->mrg.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->mrg.p;
+    cvb_register_result *rres = (cvb_register_result *)(b + o_rres);
+    cvb_register_stats *rst = (cvb_register_stats *)(b + o_rst);
+    cvb_register_match *mt = (cvb_register_match *)(b + o_m);
+    cvb_view_constraints_result *dcres = (cvb_view_constraints_result *)(b + o_cres);
+    cvb_recon_result *ores = (cvb_recon_result *)(b + o_ores);
+    cvb_incorporate_counts *cnt = (cvb_incorporate_counts *)(b + o_cnt);
+    cvb_pose *wt = (cvb_pose *)(b + o_wt), *pout = (cvb_pose *)(b + o_pout);
+    uint8_t *vs = b + o_vs, *os = b + o_os;
+    uint32_t *amap = (uint32_t *)(b + o_amap), *ltl = (uint32_t *)(b + o_ltl), *svm = (uint32_t *)(b + o_svm);
+    uint32_t *avmap = (uint32_t *)(b + o_vmap), *almap = (uint32_t *)(b + o_lmap);
+    IncSnap a = inc_snap_at(b, o, true, hc);
+    cvb_merge_result R;
+    memset(&R, 0, sizeof(R));
+    R.dest_view = CVB_MERGE_NONE;
+    std::vector<cvb_view_constraints_result> cres(VS, cvb_view_constraints_result{0, 0});
+    // 1. register_frame of s_view's frame against D
+    if ((rc = register_frame_dev(ctx, rcfg, tri, arrsac, rng, V, poses, vo, vl, bear, desc, nf, L, lo, obs, n_obs, desc_s + 64 * (size_t)r0,
+                                 bear_s + 3 * (size_t)r0, N, view_matches, H, rres, mt, nullptr, rst)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(&R.reg, rres, sizeof(cvb_register_result), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(&R.reg_stats, rst, sizeof(cvb_register_stats), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    const uint32_t M = R.reg.status == CVB_REGISTER_OK ? R.reg.n_matches : 0;
+    // the maps: dest from D, src from S; NONE unless set below
+    if (L) CVB_CUDA(ctx, cudaMemsetAsync(dlmap, 0xff, sizeof(uint32_t) * L, st));
+    CVB_CUDA(ctx, cudaMemsetAsync(dvmap, 0xff, sizeof(uint32_t) * V, st));
+    if (LS) CVB_CUDA(ctx, cudaMemsetAsync(slmap_dev, 0xff, sizeof(uint32_t) * LS, st));
+    if (VS) CVB_CUDA(ctx, cudaMemsetAsync(svmap_dev, 0xff, sizeof(uint32_t) * VS, st));
+    if (R.reg.status == CVB_REGISTER_PANIC) {
+        R.status = CVB_MERGE_REGISTER_PANIC;
+    } else if (R.reg.status != CVB_REGISTER_OK) {
+        R.status = CVB_MERGE_NOT_REGISTERED;   // D unchanged
+        IncSnap d{(cvb_pose *)poses, (uint32_t *)vo, (uint32_t *)vl, (double *)bear, (uint8_t *)desc, (uint8_t *)col, (uint32_t *)lo,
+                  (uint32_t *)obs, (cvb_view_constraint *)cons};
+        R.counts.V = V; R.counts.n_features = nf; R.counts.L = L; R.counts.n_observations = n_obs; R.counts.C = C;
+        if ((rc = inc_copy(ctx, d, R.counts, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out))) return rc;
+        k_inc_compose<<<cdiv(V, 256), 256, 0, st>>>(V, nullptr, V, nullptr, dvmap);
+        CVB_LAUNCH_CHECK(ctx);
+        if (L) {
+            k_inc_compose<<<cdiv(L, 256), 256, 0, st>>>(L, nullptr, L, nullptr, dlmap);
+            CVB_LAUNCH_CHECK(ctx);
+        }
+    } else {
+        // 2. add_view of the frame; its landmark count follows from the matches: L - merges + (N - matches)
+        std::vector<cvb_register_match> hm(M);
+        if (M) CVB_CUDA(ctx, cudaMemcpyAsync(hm.data(), mt, sizeof(cvb_register_match) * M, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        uint32_t merges = 0;
+        for (const cvb_register_match &m : hm) merges += m.landmark_b != CVB_REGISTER_NONE;
+        const uint32_t La = L - merges + (N - M);
+        if ((rc = add_view_enqueue(ctx, V, poses, vo, vl, bear, desc, col_out ? col : nullptr, nf, L, lo, obs, n_obs, &rres->pose, bear_s + 3 * (size_t)r0,
+                                   desc_s + 64 * (size_t)r0, col_out ? col_s + 3 * (size_t)r0 : nullptr, N, mt, M, a.poses, a.vo, a.vl, a.bear, a.desc,
+                                   a.col, a.lo, a.obs, amap, cnt)))
+            return rc;
+        if (C) CVB_CUDA(ctx, cudaMemcpyAsync(a.cons, cons, sizeof(cvb_view_constraint) * C, cudaMemcpyDeviceToDevice, st));
+        // 3. the dest view's constraints
+        const uint32_t q = V;
+        if ((rc = view_constraints_dev(ctx, ccfg, tri, V1, a.poses, a.vo, a.vl, a.bear, nf1, La, a.lo, a.obs, no1, &q, 1, a.cons + C, dcres, nullptr)))
+            return rc;
+        CVB_CUDA(ctx, cudaMemcpyAsync(&R.con, dcres, sizeof(cvb_view_constraints_result), cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cvb_wait(ctx, st));
+        const uint32_t Ca = C + R.con.n_constraints;
+        if (!R.con.accepted) {
+            // remove_view of the dest view: the merges stay, S is untouched
+            R.status = CVB_MERGE_REJECTED;
+            CVB_CUDA(ctx, cudaMemsetAsync(vs, CVB_RECON_VIEW_KEPT, V, st));
+            CVB_CUDA(ctx, cudaMemsetAsync(vs + V, CVB_RECON_VIEW_NO_EDGES, 1, st));
+            if (no1) {
+                k_inc_reject_states<<<cdiv(no1, 256), 256, 0, st>>>(no1, V, a.obs, os);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            if ((rc = apply_enqueue(ctx, V1, a.poses, a.vo, a.bear, a.desc, a.col, nf1, La, a.lo, a.obs, no1, a.cons, C, vs, os, poses_out, vo_out,
+                                    vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out, avmap, almap, cnt)))
+                return rc;
+            k_inc_compose<<<cdiv(V, 256), 256, 0, st>>>(V, nullptr, V1, avmap, dvmap);
+            CVB_LAUNCH_CHECK(ctx);
+            if (L) {
+                k_inc_compose<<<cdiv(L, 256), 256, 0, st>>>(L, amap, La, almap, dlmap);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            CVB_CUDA(ctx, cudaMemcpyAsync(&R.counts, cnt, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+            CVB_CUDA(ctx, cvb_wait(ctx, st));
+        } else {
+            // 4. landmark_to_landmark and the world transform
+            if (LS) CVB_CUDA(ctx, cudaMemsetAsync(ltl, 0xff, sizeof(uint32_t) * LS, st));
+            if (M) {
+                k_mg_ltl<<<cdiv(M, 256), 256, 0, st>>>(M, mt, N, vl_s + r0, LS, L, amap, ltl);
+                CVB_LAUNCH_CHECK(ctx);
+            }
+            k_mg_world<<<1, 1, 0, st>>>(&rres->pose, poses_s + s_view, wt);
+            CVB_LAUNCH_CHECK(ctx);
+            // 5. incorporate_reconstruction with s_view skipped
+            IncSnap fin;
+            const uint32_t *tgt;
+            std::vector<uint32_t> svmap;
+            if ((rc = move_and_constrain(ctx, ccfg, tri, V1, a.poses, a.vo, a.vl, a.bear, a.desc, a.col, nf1, La, a.lo, a.obs, no1, a.cons, Ca, VS,
+                                         poses_s, vo_s, vl_s, bear_s, desc_s, col_out ? col_s : nullptr, nf_s, LS, lo_s, obs_s, n_obs_s, s_view, N, wt,
+                                         ltl, fin, tgt, svmap, cres, R.move)))
+                return rc;
+            svmap[s_view] = V;
+            const cvb_incorporate_counts &f = R.move.counts;
+            // 6. optimize_reconstruction and its edits
+            if ((rc = optimize_reconstruction_dev(ctx, ocfg, tri, f.V, fin.poses, fin.vo, fin.vl, fin.bear, f.n_features, f.L, fin.lo, fin.obs,
+                                                  f.n_observations, fin.cons, f.C, ores, pout, vs, os)))
+                return rc;
+            CVB_CUDA(ctx, cudaMemcpyAsync(&R.recon, ores, sizeof(cvb_recon_result), cudaMemcpyDeviceToHost, st));
+            CVB_CUDA(ctx, cvb_wait(ctx, st));
+            if (R.recon.status == CVB_RECON_KEPT) {
+                R.status = CVB_MERGE_MERGED;
+                if ((rc = apply_enqueue(ctx, f.V, pout, fin.vo, fin.bear, fin.desc, fin.col, f.n_features, f.L, fin.lo, fin.obs, f.n_observations,
+                                        fin.cons, f.C, vs, os, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out, avmap,
+                                        almap, cnt)))
+                    return rc;
+                // D's views and landmarks kept their indices through the move: add_view's maps, then the optimisation's
+                k_inc_compose<<<cdiv(V, 256), 256, 0, st>>>(V, nullptr, f.V, avmap, dvmap);
+                CVB_LAUNCH_CHECK(ctx);
+                if (L) {
+                    k_inc_compose<<<cdiv(L, 256), 256, 0, st>>>(L, amap, f.L, almap, dlmap);
+                    CVB_LAUNCH_CHECK(ctx);
+                }
+                CVB_CUDA(ctx, cudaMemcpyAsync(svm, svmap.data(), sizeof(uint32_t) * VS, cudaMemcpyHostToDevice, st));
+                k_inc_compose<<<cdiv(VS, 256), 256, 0, st>>>(VS, svm, f.V, avmap, svmap_dev);
+                CVB_LAUNCH_CHECK(ctx);
+                if (LS) {
+                    k_inc_compose<<<cdiv(LS, 256), 256, 0, st>>>(LS, tgt, f.L, almap, slmap_dev);
+                    CVB_LAUNCH_CHECK(ctx);
+                }
+                uint32_t dv = CVB_MERGE_NONE;
+                CVB_CUDA(ctx, cudaMemcpyAsync(&R.counts, cnt, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+                CVB_CUDA(ctx, cudaMemcpyAsync(&dv, avmap + V, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+                CVB_CUDA(ctx, cvb_wait(ctx, st));
+                R.dest_view = dv;
+            } else {
+                R.status = R.recon.status == CVB_RECON_REMOVED_CONSTRAINTS ? CVB_MERGE_REMOVED_CONSTRAINTS
+                         : R.recon.status == CVB_RECON_REMOVED_FILTER      ? CVB_MERGE_REMOVED_FILTER
+                                                                           : CVB_MERGE_RECON_PANIC;
+            }
+        }
+    }
+    if (VS) CVB_CUDA(ctx, cudaMemcpyAsync(cres_dev, cres.data(), sizeof(cvb_view_constraints_result) * VS, cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(res_dev, &R, sizeof(R), cudaMemcpyHostToDevice, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+namespace {
+
+// S's snapshot (no constraints) into device rows laid out by inc_snap_layout
+int mg_upload(cvb_ctx *ctx, const IncSnap &s, uint32_t VS, const cvb_pose *poses, const uint32_t *vo, const uint32_t *vl, const double *bear,
+              const uint8_t *desc, const uint8_t *col, uint32_t LS, const uint32_t *lo, const uint32_t *obs) {
+    cudaStream_t st = ctx->stream;
+    const uint32_t nf = vo[VS], no = lo[LS];
+    const cudaMemcpyKind k = cudaMemcpyHostToDevice;
+    if (VS) CVB_CUDA(ctx, cudaMemcpyAsync(s.poses, poses, sizeof(cvb_pose) * VS, k, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(s.vo, vo, sizeof(uint32_t) * ((size_t)VS + 1), k, st));
+    if (nf) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(s.vl, vl, sizeof(uint32_t) * (size_t)nf, k, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(s.bear, bear, sizeof(double) * 3 * (size_t)nf, k, st));
+        if (desc && s.desc) CVB_CUDA(ctx, cudaMemcpyAsync(s.desc, desc, 64 * (size_t)nf, k, st));
+        if (col && s.col) CVB_CUDA(ctx, cudaMemcpyAsync(s.col, col, 3 * (size_t)nf, k, st));
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(s.lo, lo, sizeof(uint32_t) * ((size_t)LS + 1), k, st));
+    if (no) CVB_CUDA(ctx, cudaMemcpyAsync(s.obs, obs, sizeof(uint32_t) * 2 * (size_t)no, k, st));
+    return 0;
+}
+
+}  // namespace
+
+int incorporate_reconstruction(cvb_ctx *ctx, const cvb_constraints_cfg *ccfg, const cvb_triangulator *tri, uint32_t V, const cvb_pose *poses,
+                               const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t L,
+                               const uint32_t *lo, const uint32_t *obs, const cvb_view_constraint *cons, uint32_t C, uint32_t VS,
+                               const cvb_pose *poses_s, const uint32_t *vo_s, const uint32_t *vl_s, const double *bear_s, const uint8_t *desc_s,
+                               const uint8_t *col_s, uint32_t LS, const uint32_t *lo_s, const uint32_t *obs_s, uint32_t skip, const cvb_pose *wt,
+                               const uint32_t *lmap, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out,
+                               uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, uint32_t *svmap,
+                               uint32_t *slmap, cvb_view_constraints_result *cres, cvb_move_result *res) {
+    if (!ctx) return CVB_EINVAL;
+    if (!ccfg || !tri || !poses || !poses_s || !wt || !poses_out || !vo_out || !lo_out || !cons_out || !res || (LS && (!lmap || !slmap)) ||
+        (VS && (!svmap || !cres)))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    static const uint32_t no_entries = 0;   // a map of L_S = 0 entries
+    if (merge_check(V, vo, vl, L, lo, obs, cons, C, VS, vo_s, vl_s, LS, lo_s, obs_s, skip, lmap ? lmap : &no_entries, col != nullptr,
+                    col_s != nullptr))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshots, skip_view or landmark map");
+    const uint32_t nf = vo[V], no = lo[L], nf_s = vo_s[VS], no_s = lo_s[LS];
+    if ((nf && (!bear || !vl_out || !bear_out)) || (nf_s && (!bear_s || !vl_out || !bear_out)) || (no + nf_s && !obs_out))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!desc != !desc_out)) || (nf_s && (!desc_s != !desc_out)) || (nf && (!col != !col_out)) || (nf_s && (!col_s != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "descriptors and colours go with both snapshots and the output together");
+    const bool hd = desc_out != nullptr, hc = col_out != nullptr;
+    const uint32_t maxc = ccfg->optimization_maximum_three_view_constraints;
+    size_t x = 0, os_[9], o[9];
+    const size_t i_wt = x; x += con_align(sizeof(cvb_pose));
+    const size_t i_lm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t i_svm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(VS, 1));
+    const size_t i_slm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t i_cr = x; x += con_align(sizeof(cvb_view_constraints_result) * std::max<size_t>(VS, 1));
+    const size_t i_res = x; x += con_align(sizeof(cvb_move_result));
+    x = inc_snap_layout(x, VS, nf_s, LS, no_s, 0, hd, hc, os_);
+    x = inc_snap_layout(x, V + VS, nf + nf_s, L + nf_s, no + nf_s, C + VS * maxc, hd, hc, o);
+    IncSnap s;
+    unsigned char *b;
+    size_t end;
+    int rc;
+    if ((rc = inc_upload(ctx, V, poses, vo, vl, bear, hd ? desc : nullptr, hc ? col : nullptr, L, lo, obs, cons, C, x, s, b, end))) return rc;
+    unsigned char *e = b + end;
+    cudaStream_t st = ctx->stream;
+    IncSnap ss = inc_snap_at(e, os_, hd, hc), out = inc_snap_at(e, o, hd, hc);
+    if ((rc = mg_upload(ctx, ss, VS, poses_s, vo_s, vl_s, bear_s, desc_s, col_s, LS, lo_s, obs_s))) return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(e + i_wt, wt, sizeof(cvb_pose), cudaMemcpyHostToDevice, st));
+    if (LS) CVB_CUDA(ctx, cudaMemcpyAsync(e + i_lm, lmap, sizeof(uint32_t) * LS, cudaMemcpyHostToDevice, st));
+    if ((rc = incorporate_reconstruction_dev(ctx, ccfg, tri, V, s.poses, s.vo, s.vl, s.bear, s.desc, s.col, nf, L, s.lo, s.obs, no, s.cons, C, VS,
+                                             ss.poses, ss.vo, ss.vl, ss.bear, ss.desc, ss.col, nf_s, LS, ss.lo, ss.obs, no_s, skip,
+                                             (const cvb_pose *)(e + i_wt), (const uint32_t *)(e + i_lm), out.poses, out.vo, out.vl, out.bear,
+                                             out.desc, out.col, out.lo, out.obs, out.cons, (uint32_t *)(e + i_svm), (uint32_t *)(e + i_slm),
+                                             (cvb_view_constraints_result *)(e + i_cr), (cvb_move_result *)(e + i_res))))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, e + i_res, sizeof(cvb_move_result), cudaMemcpyDeviceToHost, st));
+    if (VS) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(svmap, e + i_svm, sizeof(uint32_t) * VS, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(cres, e + i_cr, sizeof(cvb_view_constraints_result) * VS, cudaMemcpyDeviceToHost, st));
+    }
+    if (LS) CVB_CUDA(ctx, cudaMemcpyAsync(slmap, e + i_slm, sizeof(uint32_t) * LS, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return inc_download(ctx, out, res->counts, hd, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
+}
+
+int merge_reconstructions(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_constraints_cfg *ccfg, const cvb_recon_cfg *ocfg,
+                          const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rng, uint32_t V, const cvb_pose *poses,
+                          const uint32_t *vo, const uint32_t *vl, const double *bear, const uint8_t *desc, const uint8_t *col, uint32_t L,
+                          const uint32_t *lo, const uint32_t *obs, const cvb_view_constraint *cons, uint32_t C, uint32_t VS, const cvb_pose *poses_s,
+                          const uint32_t *vo_s, const uint32_t *vl_s, const double *bear_s, const uint8_t *desc_s, const uint8_t *col_s, uint32_t LS,
+                          const uint32_t *lo_s, const uint32_t *obs_s, uint32_t s_view, const uint32_t *view_matches, uint32_t H,
+                          cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out,
+                          uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, uint32_t *dvmap, uint32_t *dlmap, uint32_t *svmap,
+                          uint32_t *slmap, cvb_view_constraints_result *cres, cvb_merge_result *res) {
+    if (!ctx) return CVB_EINVAL;
+    if (!rcfg || !ccfg || !ocfg || !tri || !arrsac || !rng || !poses || !poses_s || !res || !poses_out || !vo_out || !lo_out || !cons_out ||
+        !dvmap || (L && !dlmap) || (VS && (!svmap || !cres)) || (LS && !slmap))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (merge_check(V, vo, vl, L, lo, obs, cons, C, VS, vo_s, vl_s, LS, lo_s, obs_s, s_view, nullptr, col != nullptr, col_s != nullptr) ||
+        register_check(V, vo, vl, L, lo, obs, view_matches, H))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed snapshots, s_view or view matches");
+    const uint32_t nf = vo[V], no = lo[L], nf_s = vo_s[VS], no_s = lo_s[LS];
+    if ((nf && (!bear || !desc)) || (nf_s && (!bear_s || !desc_s)) || (nf + nf_s && (!vl_out || !bear_out || !desc_out)) || (no + nf_s && !obs_out))
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if ((nf && (!col != !col_out)) || (nf_s && (!col_s != !col_out)))
+        return cvb_set_error(ctx, CVB_EINVAL, "colours go with both snapshots and the output together");
+    const bool hc = col_out != nullptr;
+    const uint32_t maxc = ccfg->optimization_maximum_three_view_constraints;
+    size_t x = 0, os_[9], o[9];
+    const size_t i_dvm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(V, 1));
+    const size_t i_dlm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(L, 1));
+    const size_t i_svm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(VS, 1));
+    const size_t i_slm = x; x += con_align(sizeof(uint32_t) * std::max<size_t>(LS, 1));
+    const size_t i_cr = x; x += con_align(sizeof(cvb_view_constraints_result) * std::max<size_t>(VS, 1));
+    const size_t i_res = x; x += con_align(sizeof(cvb_merge_result));
+    x = inc_snap_layout(x, VS, nf_s, LS, no_s, 0, true, hc, os_);
+    x = inc_snap_layout(x, V + VS, nf + nf_s, L + no + 4 * nf_s, no + 2 * nf_s, C + (VS + 1) * maxc, true, hc, o);
+    IncSnap s;
+    unsigned char *b;
+    size_t end;
+    int rc;
+    if ((rc = inc_upload(ctx, V, poses, vo, vl, bear, desc, hc ? col : nullptr, L, lo, obs, cons, C, x, s, b, end))) return rc;
+    unsigned char *e = b + end;
+    cudaStream_t st = ctx->stream;
+    IncSnap ss = inc_snap_at(e, os_, true, hc), out = inc_snap_at(e, o, true, hc);
+    if ((rc = mg_upload(ctx, ss, VS, poses_s, vo_s, vl_s, bear_s, desc_s, hc ? col_s : nullptr, LS, lo_s, obs_s))) return rc;
+    cvb_merge_result *rd = (cvb_merge_result *)(e + i_res);
+    if ((rc = merge_reconstructions_dev(ctx, rcfg, ccfg, ocfg, tri, arrsac, rng, V, s.poses, s.vo, s.vl, s.bear, s.desc, s.col, nf, L, s.lo, s.obs, no,
+                                        s.cons, C, VS, ss.poses, ss.vo, ss.vl, ss.bear, ss.desc, ss.col, nf_s, LS, ss.lo, ss.obs, no_s, s_view,
+                                        view_matches, H, out.poses, out.vo, out.vl, out.bear, out.desc, out.col, out.lo, out.obs, out.cons,
+                                        (uint32_t *)(e + i_dvm), (uint32_t *)(e + i_dlm), (uint32_t *)(e + i_svm), (uint32_t *)(e + i_slm),
+                                        (cvb_view_constraints_result *)(e + i_cr), rd)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, rd, sizeof(cvb_merge_result), cudaMemcpyDeviceToHost, st));
+    if (V) CVB_CUDA(ctx, cudaMemcpyAsync(dvmap, e + i_dvm, sizeof(uint32_t) * V, cudaMemcpyDeviceToHost, st));
+    if (L) CVB_CUDA(ctx, cudaMemcpyAsync(dlmap, e + i_dlm, sizeof(uint32_t) * L, cudaMemcpyDeviceToHost, st));
+    if (VS) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(svmap, e + i_svm, sizeof(uint32_t) * VS, cudaMemcpyDeviceToHost, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(cres, e + i_cr, sizeof(cvb_view_constraints_result) * VS, cudaMemcpyDeviceToHost, st));
+    }
+    if (LS) CVB_CUDA(ctx, cudaMemcpyAsync(slmap, e + i_slm, sizeof(uint32_t) * LS, cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    const bool have = res->status == CVB_MERGE_MERGED || res->status == CVB_MERGE_REJECTED || res->status == CVB_MERGE_NOT_REGISTERED;
+    if (!have) return 0;
     return inc_download(ctx, out, res->counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
 }
 

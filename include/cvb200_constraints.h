@@ -48,7 +48,8 @@
  * up to these orders.
  *
  * A call over every view equals regenerate_reconstruction's constraint pass (lib.rs:2418-2435), which removes nothing.
- * incorporate_reconstruction removes views between its calls to record_view_constraints, so it can use this call one view at a time. */
+ * incorporate_reconstruction removes views between its calls to record_view_constraints; include/cvb200_merge.h runs it as one call over
+ * every moved view, repeated after each refusal for the views after it, which gives the results of the one-view-at-a-time loop. */
 #ifndef CVB200_CONSTRAINTS_H
 #define CVB200_CONSTRAINTS_H
 #include "cvb200.h"
