@@ -225,3 +225,6 @@ pub mod incorporate;
 
 // ---- INTEGRATION.md section 2r (include/cvb200_merge.h) ----
 pub mod merge;
+
+// ---- INTEGRATION.md section 2s (include/cvb200_try_init.h) ----
+pub mod try_init;

@@ -35,6 +35,8 @@ Host-side mirror of the reference's interfaces for this path, over the C ABI in 
                            (cv-sfm/src/lib.rs:432-588, 699-721, 2067-2087): one reconstruction snapshot to the next, on the device
   incorporate_reconstruction, merge_reconstructions <- cv-sfm VSlam::incorporate_reconstruction and try_merge_reconstructions followed
                            by optimize_reconstruction (cv-sfm/src/lib.rs:1817-1887, 2116-2193): two reconstruction snapshots to one
+  add_reconstruction, try_init <- cv-sfm VSlamData::add_reconstruction and VSlam::try_init (cv-sfm/src/lib.rs:377-427, 814-839): a frame
+                           and its free frames to the first snapshot of a new reconstruction
   *Triangulator         <- cv-geom's six triangulators          (cv-geom/src/triangulation.rs)
   *_optimize_l1/_l2     <- cv-optimize's five pose optimizers   (cv-optimize/src/{single,three}_view_optimizer.rs)
 
@@ -68,5 +70,6 @@ from .export import ExportSettings, export_reconstruction, normalize_reconstruct
 from .register import RegisterSettings, register_frame  # noqa: F401
 from .incorporate import add_view, apply_optimization, incorporate_frame  # noqa: F401
 from .merge import incorporate_reconstruction, incorporate_reconstruction_dev, merge_reconstructions, merge_reconstructions_dev  # noqa: F401
+from .try_init import add_reconstruction, add_reconstruction_dev, try_init, try_init_dev  # noqa: F401
 
 __version__ = "0.1.0"

@@ -4,8 +4,8 @@ cv_b200/libcvb200_opt.so (include/cvb200_opt.h), cv_b200/libcvb200_pinhole.so (i
 cv_b200/libcvb200_stages.so (include/cvb200_stages.h), cv_b200/libcvb200_batch.so (include/cvb200_batch.h), cv_b200/libcvb200_init.so
 (include/cvb200_init.h), cv_b200/libcvb200_constraints.so (include/cvb200_constraints.h), cv_b200/libcvb200_reconstruction.so
 (include/cvb200_reconstruction.h), cv_b200/libcvb200_export.so (include/cvb200_export.h) and
-cv_b200/libcvb200_register.so (include/cvb200_register.h), cv_b200/libcvb200_incorporate.so (include/cvb200_incorporate.h) and
-cv_b200/libcvb200_merge.so (include/cvb200_merge.h)."""
+cv_b200/libcvb200_register.so (include/cvb200_register.h), cv_b200/libcvb200_incorporate.so (include/cvb200_incorporate.h),
+cv_b200/libcvb200_merge.so (include/cvb200_merge.h) and cv_b200/libcvb200_try_init.so (include/cvb200_try_init.h)."""
 import ctypes as C
 import os
 
@@ -151,6 +151,9 @@ INCORPORATE_ABI_SYMBOLS = ["cvb_incorporate_check", "cvb_add_view_dev", "cvb_add
 # tests/test_abi_merge.py
 MERGE_ABI_SYMBOLS = ["cvb_merge_check", "cvb_incorporate_reconstruction_dev", "cvb_incorporate_reconstruction", "cvb_merge_reconstructions_dev",
                      "cvb_merge_reconstructions"]
+# every symbol include/cvb200_try_init.h declares (cv-sfm's reconstruction creation), exported by libcvb200_try_init.so; checked by
+# tests/test_abi_try_init.py
+TRY_INIT_ABI_SYMBOLS = ["cvb_try_init_check", "cvb_add_reconstruction_dev", "cvb_add_reconstruction", "cvb_try_init_dev", "cvb_try_init"]
 
 # cvb_akaze_evolution: the scalar fields of akaze's EvolutionStep (evolution.rs:8-44), level size and FED step count
 EVOLUTION_DTYPE = np.dtype([("octave", "<u4"), ("sublevel", "<u4"), ("esigma", "<f8"), ("etime", "<f8"), ("sigma_size", "<u4"),
@@ -552,6 +555,32 @@ def load_merge_library():
                                                 [u32, vp, vp, u32, vp, u32] + [vp] * 15)
         _MERGE_LIB = L
     return _MERGE_LIB
+
+
+_TRY_INIT_LIB = None
+
+
+def try_init_lib_path():
+    return os.path.join(_HERE, "libcvb200_try_init.so")
+
+
+def load_try_init_library():
+    """Loads libcvb200_try_init.so, the module of include/cvb200_try_init.h over libcvb200.so (same contexts). Fails loudly when missing."""
+    global _TRY_INIT_LIB
+    if _TRY_INIT_LIB is None:
+        load_library()
+        p = try_init_lib_path()
+        if not os.path.exists(p):
+            raise CvbError(CVB_ENODEV, f"{p} not built: run `make -C cv_b200/csrc`")
+        L = C.CDLL(p)
+        vp, u32 = C.c_void_p, C.c_uint32
+        L.cvb_try_init_check.argtypes = [u32] * 6 + [vp, u32, vp, u32, vp, u32]
+        L.cvb_add_reconstruction_dev.argtypes = [vp] * 5 + [u32] * 5 + [vp] * 14
+        L.cvb_add_reconstruction.argtypes = [vp] * 5 + [u32] * 5 + [vp] * 14
+        L.cvb_try_init_dev.argtypes = [vp] * 5 + [u32] + [vp] * 4 + [u32] * 3 + [vp, u32] + [vp] * 10
+        L.cvb_try_init.argtypes = [vp] * 5 + [u32] + [vp] * 4 + [u32] * 3 + [vp, u32] + [vp] * 10
+        _TRY_INIT_LIB = L
+    return _TRY_INIT_LIB
 
 
 class Context:

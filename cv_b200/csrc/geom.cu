@@ -26,6 +26,7 @@
 #include "../../include/cvb200_register.h"
 #include "../../include/cvb200_incorporate.h"
 #include "../../include/cvb200_merge.h"
+#include "../../include/cvb200_try_init.h"
 #include "c2c_filter.cuh"
 #include "pinhole.cuh"
 
@@ -1583,6 +1584,7 @@ __global__ void __launch_bounds__(128) k_tri_landmark_robust(cvb_triangulator T,
 #include "register_dev.cuh"
 #include "incorporate_dev.cuh"
 #include "merge_dev.cuh"
+#include "try_init_dev.cuh"
 
 // ------------------------------------------------------------------------------------------ cv-pinhole (include/cvb200_pinhole.h)
 // cv-pinhole/src/lib.rs:314-372 pose_reprojection_error + average_pose_reprojection_error of one FeatureMatch.  Kept from the reference:
@@ -1747,12 +1749,14 @@ struct GeomWorkspace {
     DevBuf reg;                     // frame registration's workspace (register_frame_dev)
     DevBuf inc, incs;               // frame incorporation's snapshot after add_view and the two edits' scratch (incorporate_frame_dev)
     DevBuf mrg, mrgs;               // merging's snapshot after add_view, and the move's snapshots and scratch (merge_dev.cuh's drivers)
+    DevBuf tinit, tinits;           // creation's add_reconstruction scratch, and try_init's two-view outputs, init result and lists
     ArsWorkspace *ars = nullptr;
 };
 void geom_workspace_free(GeomWorkspace *g) {
     if (!g) return;
     DevBuf *bufs[] = {&g->a, &g->b, &g->samples, &g->poses, &g->nposes, &g->out, &g->masks, &g->offsets, &g->ok, &g->init, &g->con,
-                      &g->con2, &g->rec, &g->exp, &g->reg, &g->inc, &g->incs, &g->mrg, &g->mrgs};
+                      &g->con2, &g->rec, &g->exp, &g->reg, &g->inc, &g->incs, &g->mrg, &g->mrgs,
+                      &g->tinit, &g->tinits};
     for (DevBuf *d : bufs) if (d->p) cudaFree(d->p);
     if (g->ars) {
         ArsWorkspace *w = g->ars;
@@ -5137,6 +5141,272 @@ int merge_reconstructions(cvb_ctx *ctx, const cvb_register_cfg *rcfg, const cvb_
     CVB_CUDA(ctx, cvb_wait(ctx, st));
     const bool have = res->status == CVB_MERGE_MERGED || res->status == CVB_MERGE_REJECTED || res->status == CVB_MERGE_NOT_REGISTERED;
     if (!have) return 0;
+    return inc_download(ctx, out, res->counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
+}
+
+// ---- cv-sfm's reconstruction creation (C names in try_init_abi.cu, include/cvb200_try_init.h; kernels in try_init_dev.cuh) -------------
+int try_init_check(uint32_t nc, uint32_t n1, uint32_t n2, uint32_t center, uint32_t first, uint32_t second, const uint32_t *comb, uint32_t K,
+                   const uint32_t *fm, uint32_t K1, const uint32_t *sm, uint32_t K2) {
+    if (center == first || center == second || first == second) return CVB_EINVAL;
+    if ((K && !comb) || (K1 && !fm) || (K2 && !sm)) return CVB_EINVAL;
+    // view col (1 or 2): every entry in range, each of its features and each center feature mapped into it at most once (HashMap::insert
+    // would otherwise drop an entry or an observation)
+    auto view = [&](uint32_t n, const uint32_t *m, uint32_t M, uint32_t col) {
+        std::vector<uint8_t> fu(n, 0), cu(nc, 0);
+        auto add = [&](uint32_t c, uint32_t f) {
+            if (c >= nc || f >= n || fu[f] || cu[c]) return false;
+            fu[f] = cu[c] = 1;
+            return true;
+        };
+        for (uint32_t i = 0; i < M; i++)
+            if (!add(m[2 * (size_t)i], m[2 * (size_t)i + 1])) return false;
+        for (uint32_t i = 0; i < K; i++)
+            if (!add(comb[3 * (size_t)i], comb[3 * (size_t)i + col])) return false;
+        return true;
+    };
+    return view(n1, fm, K1, 1) && view(n2, sm, K2, 2) ? 0 : CVB_EINVAL;
+}
+
+namespace {
+
+// the refusals of the frame indices every entry shares
+int ti_frames(cvb_ctx *ctx, uint32_t frames, uint32_t cap, uint32_t center, uint32_t first, uint32_t second) {
+    if (cap == 0) return cvb_set_error(ctx, CVB_EINVAL, "zero capacity");
+    if (center >= frames || first >= frames || second >= frames)
+        return cvb_set_error(ctx, CVB_EINVAL, "frames %u, %u, %u of %u", center, first, second, frames);
+    if (center == first || center == second || first == second) return cvb_set_error(ctx, CVB_EINVAL, "two equal frames");
+    return 0;
+}
+
+// a grid of at most 64 CTAs of 256 threads: the rows are few, and every try_init_dev.cuh kernel strides past the grid
+uint32_t ti_grid(uint32_t n) { return std::max<uint32_t>(std::min<uint32_t>(cdiv(n, 256), 64), 1); }
+
+// add_reconstruction enqueued on the context's stream (no wait); scratch in the context's creation scratch buffer
+int add_reconstruction_enqueue(cvb_ctx *ctx, const uint8_t *desc, const uint32_t *n, const double *bear, const uint8_t *col, uint32_t cap,
+                               TiFrames fr, const cvb_init_result *ir, const uint32_t *comb, const uint32_t *fm, const uint32_t *sm,
+                               cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out, uint8_t *col_out,
+                               uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, cvb_incorporate_counts *counts) {
+    const uint32_t n3 = 3 * cap;
+    size_t off = 0;
+    const size_t o_maps = off; off += con_align(sizeof(uint32_t) * 4 * (size_t)cap);
+    const size_t o_cnt = off; off += con_align(sizeof(uint2) * (size_t)n3);
+    const size_t o_tiles = off; off += con_align(sizeof(uint2) * (size_t)cdiv(n3, INC_TILE));
+    const size_t o_total = off; off += con_align(sizeof(uint2));
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->tinit.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->tinit.p;
+    uint32_t *maps = (uint32_t *)(b + o_maps), *fmap1 = maps, *fmap2 = maps + cap, *cmap1 = maps + 2 * (size_t)cap, *cmap2 = maps + 3 * (size_t)cap;
+    uint2 *cnt = (uint2 *)(b + o_cnt), *tiles = (uint2 *)(b + o_tiles), *total = (uint2 *)(b + o_total);
+    cudaStream_t st = ctx->stream;
+    CVB_PROF(ctx, "k_ti", 0);
+    k_ti_clear<<<ti_grid(4 * cap), 256, 0, st>>>(4 * cap, maps);
+    CVB_LAUNCH_CHECK(ctx);
+    k_ti_map<<<ti_grid(cap), 256, 0, st>>>(cap, fr, n, ir, comb, fm, sm, fmap1, fmap2, cmap1, cmap2);
+    CVB_LAUNCH_CHECK(ctx);
+    k_ti_counts<<<ti_grid(n3), 256, 0, st>>>(cap, fr, n, fmap1, fmap2, cmap1, cmap2, cnt);
+    CVB_LAUNCH_CHECK(ctx);
+    if ((rc = inc_scan(ctx, n3, cnt, tiles, total))) return rc;
+    k_ti_place<<<ti_grid(n3), 256, 0, st>>>(cap, fr, n, bear, (const uint4 *)desc, col, fmap1, fmap2, cmap1, cmap2, cnt, vl_out, bear_out,
+                                            (uint4 *)desc_out, col_out, lo_out, obs_out);
+    CVB_LAUNCH_CHECK(ctx);
+    k_ti_finish<<<1, 1, 0, st>>>(cap, fr, n, ir, total, poses_out, vo_out, lo_out, cons_out, counts);
+    CVB_LAUNCH_CHECK(ctx);
+    return 0;
+}
+
+}  // namespace
+
+int add_reconstruction_dev(cvb_ctx *ctx, const uint8_t *desc, const uint32_t *n, const double *bear, const uint8_t *col, uint32_t frames,
+                           uint32_t cap, uint32_t center, uint32_t first, uint32_t second, const cvb_init_result *ir, const uint32_t *comb,
+                           const uint32_t *fm, const uint32_t *sm, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out,
+                           uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out,
+                           cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!desc || !n || !bear || !ir || !comb || !fm || !sm || !poses_out || !vo_out || !vl_out || !bear_out || !desc_out || !lo_out || !obs_out ||
+        !cons_out || !counts)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (!col != !col_out) return cvb_set_error(ctx, CVB_EINVAL, "colours go with the frame store and the output together");
+    int rc;
+    if ((rc = ti_frames(ctx, frames, cap, center, first, second))) return rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = add_reconstruction_enqueue(ctx, desc, n, bear, col, cap, TiFrames{{center, first, second}}, ir, comb, fm, sm, poses_out, vo_out,
+                                         vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out, counts)))
+        return rc;
+    CVB_CUDA(ctx, cvb_wait(ctx, ctx->stream));
+    return 0;
+}
+
+int try_init_dev(cvb_ctx *ctx, const cvb_init_cfg *icfg, const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rngs,
+                 uint32_t better_by, const uint8_t *desc, const uint32_t *n, const double *bear, const uint8_t *col, uint32_t frames, uint32_t cap,
+                 uint32_t center, const uint32_t *options, uint32_t F, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out,
+                 uint8_t *desc_out, uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out,
+                 cvb_try_init_result *res_dev) {
+    if (!ctx) return CVB_EINVAL;
+    if (!icfg || !tri || !arrsac || (F && (!rngs || !options)) || !desc || !n || !bear || !poses_out || !vo_out || !vl_out || !bear_out ||
+        !desc_out || !lo_out || !obs_out || !cons_out || !res_dev)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (!col != !col_out) return cvb_set_error(ctx, CVB_EINVAL, "colours go with the frame store and the output together");
+    if (F > CVB_ARRSAC_BATCH_MAX) return cvb_set_error(ctx, CVB_EUNSUPPORTED, "%u options: at most %u", F, CVB_ARRSAC_BATCH_MAX);
+    if (tri->method < CVB_TRI_LINEAR_EIGEN || tri->method > CVB_TRI_MEAN_MEAN)
+        return cvb_set_error(ctx, tri->method >= CVB_TRI_RELATIVE_DLT && tri->method <= CVB_TRI_ANGULAR_LINF ? CVB_EUNSUPPORTED : CVB_EINVAL,
+                             "triangulator method %d: try_init takes a TriangulatorObservations (methods 0-2)", tri->method);
+    if (cap == 0) return cvb_set_error(ctx, CVB_EINVAL, "zero capacity");
+    if (center >= frames) return cvb_set_error(ctx, CVB_EINVAL, "center frame %u of %u", center, frames);
+    for (uint32_t f = 0; f < F; f++)
+        if (options[f] >= frames) return cvb_set_error(ctx, CVB_EINVAL, "option %u: frame %u of %u", f, options[f], frames);
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    // the two-view outputs and the init's result and lists stay in the context's creation buffer
+    const uint32_t Fm = std::max<uint32_t>(F, 1);
+    size_t off = 0;
+    const size_t o_pairs = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)Fm * cap);
+    const size_t o_np = off; off += con_align(sizeof(uint32_t) * Fm);
+    const size_t o_model = off; off += con_align(sizeof(cvb_pose) * Fm);
+    const size_t o_inl = off; off += con_align(sizeof(uint32_t) * (size_t)Fm * cap);
+    const size_t o_ninl = off; off += con_align(sizeof(uint32_t) * Fm);
+    const size_t o_found = off; off += con_align(sizeof(int32_t) * Fm);
+    const size_t o_ir = off; off += con_align(sizeof(cvb_init_result));
+    const size_t o_comb = off; off += con_align(sizeof(uint32_t) * 3 * (size_t)cap);
+    const size_t o_fm = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)cap);
+    const size_t o_sm = off; off += con_align(sizeof(uint32_t) * 2 * (size_t)cap);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    if ((rc = g->tinits.ensure(ctx, off))) return rc;
+    unsigned char *b = (unsigned char *)g->tinits.p;
+    uint32_t *pairs = (uint32_t *)(b + o_pairs), *np = (uint32_t *)(b + o_np), *inl = (uint32_t *)(b + o_inl), *ninl = (uint32_t *)(b + o_ninl);
+    cvb_pose *model = (cvb_pose *)(b + o_model);
+    int32_t *found = (int32_t *)(b + o_found);
+    cvb_init_result *ir = (cvb_init_result *)(b + o_ir);
+    uint32_t *comb = (uint32_t *)(b + o_comb), *fm = (uint32_t *)(b + o_fm), *sm = (uint32_t *)(b + o_sm);
+    cudaStream_t st = ctx->stream;
+    if (F) {
+        if ((rc = two_view_options_dev(ctx, desc, n, bear, frames, cap, center, options, F, better_by, arrsac, rngs, pairs, np, model, inl, ninl,
+                                       found)))
+            return rc;
+        if ((rc = ars_commit_rng_batch(ctx, rngs, F, nullptr))) return rc;
+    }
+    if ((rc = init_reconstruction_dev(ctx, icfg, tri, bear, frames, cap, center, options, F, pairs, np, model, inl, ninl, found, ir, comb, fm, sm,
+                                      nullptr)))
+        return rc;
+    cvb_init_result *h = (cvb_init_result *)cvb_pinned(ctx, sizeof(cvb_init_result));
+    if (!h) return cvb_set_error(ctx, CVB_ENOMEM, "page-locked scratch");
+    CVB_CUDA(ctx, cudaMemcpyAsync(h, ir, sizeof(cvb_init_result), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    cvb_try_init_result R;
+    memset(&R, 0, sizeof(R));
+    R.init = *h;
+    R.status = R.init.status == CVB_INIT_ACCEPTED ? CVB_TRY_INIT_CREATED
+                                                  : (R.init.status == CVB_INIT_NONE_BEARING_PAIRS ? CVB_TRY_INIT_NONE_BEARING_PAIRS : CVB_TRY_INIT_NONE);
+    R.frames[0] = center;
+    R.frames[1] = R.frames[2] = CVB_TRY_INIT_NO_FRAME;
+    if (R.init.status != CVB_INIT_NONE && R.init.first < F && R.init.second < F) {
+        R.frames[1] = options[R.init.first];
+        R.frames[2] = options[R.init.second];
+    }
+    // the record first, then (created) the snapshot, whose counts the placement writes into it
+    CVB_CUDA(ctx, cudaMemcpyAsync(res_dev, &R, sizeof(R), cudaMemcpyHostToDevice, st));
+    if (R.status == CVB_TRY_INIT_CREATED &&
+        (rc = add_reconstruction_enqueue(ctx, desc, n, bear, col, cap, TiFrames{{R.frames[0], R.frames[1], R.frames[2]}}, ir, comb, fm, sm,
+                                         poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out, &res_dev->counts)))
+        return rc;
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return 0;
+}
+
+int add_reconstruction(cvb_ctx *ctx, const uint8_t *desc, const uint32_t *n, const double *bear, const uint8_t *col, uint32_t frames, uint32_t cap,
+                       uint32_t center, uint32_t first, uint32_t second, const cvb_init_result *ir, const uint32_t *comb, const uint32_t *fm,
+                       const uint32_t *sm, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out,
+                       uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, cvb_incorporate_counts *counts) {
+    if (!ctx) return CVB_EINVAL;
+    if (!desc || !n || !bear || !ir || !poses_out || !vo_out || !vl_out || !bear_out || !desc_out || !lo_out || !obs_out || !cons_out || !counts)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (!col != !col_out) return cvb_set_error(ctx, CVB_EINVAL, "colours go with the frame store and the output together");
+    int rc;
+    if ((rc = ti_frames(ctx, frames, cap, center, first, second))) return rc;
+    const uint32_t fr[3] = {center, first, second}, K = ir->n_combined, K1 = ir->n_first_matches, K2 = ir->n_second_matches;
+    if (try_init_check(std::min(n[center], cap), std::min(n[first], cap), std::min(n[second], cap), center, first, second, comb, K, fm, K1, sm, K2))
+        return cvb_set_error(ctx, CVB_EINVAL, "malformed match lists");
+    // the three frames as a store of three, the result and the lists uploaded; the outputs after them
+    const bool hc = col != nullptr;
+    size_t x = 0, o[9];
+    const size_t i_desc = x; x += con_align(64 * 3 * (size_t)cap);
+    const size_t i_bear = x; x += con_align(sizeof(double) * 9 * (size_t)cap);
+    const size_t i_col = x; x += hc ? con_align(9 * (size_t)cap) : 0;
+    const size_t i_n = x; x += con_align(sizeof(uint32_t) * 3);
+    const size_t i_ir = x; x += con_align(sizeof(cvb_init_result));
+    const size_t i_comb = x; x += con_align(sizeof(uint32_t) * 3 * (size_t)cap);
+    const size_t i_fm = x; x += con_align(sizeof(uint32_t) * 2 * (size_t)cap);
+    const size_t i_sm = x; x += con_align(sizeof(uint32_t) * 2 * (size_t)cap);
+    const size_t i_cnt = x; x += con_align(sizeof(cvb_incorporate_counts));
+    x = inc_snap_layout(x, 3, 3 * cap, 3 * cap, 3 * cap, 1, true, hc, o);
+    GeomWorkspace *g = gws(ctx);
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = g->out.ensure(ctx, x))) return rc;
+    unsigned char *b = (unsigned char *)g->out.p;
+    IncSnap out = inc_snap_at(b, o, true, hc);
+    cudaStream_t st = ctx->stream;
+    const cudaMemcpyKind k = cudaMemcpyHostToDevice;
+    uint32_t n3[3];
+    for (int v = 0; v < 3; v++) {
+        n3[v] = std::min(n[fr[v]], cap);
+        const size_t s = (size_t)fr[v] * cap;
+        CVB_CUDA(ctx, cudaMemcpyAsync(b + i_desc + 64 * (size_t)v * cap, desc + 64 * s, 64 * (size_t)n3[v], k, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(b + i_bear + sizeof(double) * 3 * (size_t)v * cap, bear + 3 * s, sizeof(double) * 3 * (size_t)n3[v], k, st));
+        if (hc) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_col + 3 * (size_t)v * cap, col + 3 * s, 3 * (size_t)n3[v], k, st));
+    }
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_n, n3, sizeof(n3), k, st));
+    CVB_CUDA(ctx, cudaMemcpyAsync(b + i_ir, ir, sizeof(cvb_init_result), k, st));
+    if (K) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_comb, comb, sizeof(uint32_t) * 3 * (size_t)K, k, st));
+    if (K1) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_fm, fm, sizeof(uint32_t) * 2 * (size_t)K1, k, st));
+    if (K2) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_sm, sm, sizeof(uint32_t) * 2 * (size_t)K2, k, st));
+    if ((rc = add_reconstruction_enqueue(ctx, b + i_desc, (const uint32_t *)(b + i_n), (const double *)(b + i_bear), hc ? b + i_col : nullptr, cap,
+                                         TiFrames{{0, 1, 2}}, (const cvb_init_result *)(b + i_ir), (const uint32_t *)(b + i_comb),
+                                         (const uint32_t *)(b + i_fm), (const uint32_t *)(b + i_sm), out.poses, out.vo, out.vl, out.bear, out.desc,
+                                         out.col, out.lo, out.obs, out.cons, (cvb_incorporate_counts *)(b + i_cnt))))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(counts, b + i_cnt, sizeof(cvb_incorporate_counts), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    return inc_download(ctx, out, *counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
+}
+
+int try_init(cvb_ctx *ctx, const cvb_init_cfg *icfg, const cvb_triangulator *tri, const cvb_arrsac_cfg *arrsac, cvb_rng *rngs, uint32_t better_by,
+             const uint8_t *desc, const uint32_t *n, const double *bear, const uint8_t *col, uint32_t frames, uint32_t cap, uint32_t center,
+             const uint32_t *options, uint32_t F, cvb_pose *poses_out, uint32_t *vo_out, uint32_t *vl_out, double *bear_out, uint8_t *desc_out,
+             uint8_t *col_out, uint32_t *lo_out, uint32_t *obs_out, cvb_view_constraint *cons_out, cvb_try_init_result *res) {
+    if (!ctx) return CVB_EINVAL;
+    if (!desc || !n || !bear || !res || !poses_out || !vo_out || !vl_out || !bear_out || !desc_out || !lo_out || !obs_out || !cons_out)
+        return cvb_set_error(ctx, CVB_EINVAL, "null argument");
+    if (!col != !col_out) return cvb_set_error(ctx, CVB_EINVAL, "colours go with the frame store and the output together");
+    const bool hc = col != nullptr;
+    const size_t rows = (size_t)frames * cap;
+    size_t x = 0, o[9];
+    const size_t i_desc = x; x += con_align(64 * std::max<size_t>(rows, 1));
+    const size_t i_bear = x; x += con_align(sizeof(double) * 3 * std::max<size_t>(rows, 1));
+    const size_t i_col = x; x += hc ? con_align(3 * std::max<size_t>(rows, 1)) : 0;
+    const size_t i_n = x; x += con_align(sizeof(uint32_t) * std::max<uint32_t>(frames, 1));
+    const size_t i_res = x; x += con_align(sizeof(cvb_try_init_result));
+    x = inc_snap_layout(x, 3, 3 * cap, 3 * cap, 3 * cap, 1, true, hc, o);
+    GeomWorkspace *g = gws(ctx);
+    int rc;
+    CVB_CUDA(ctx, cudaSetDevice(ctx->device));
+    if ((rc = g->out.ensure(ctx, x))) return rc;
+    unsigned char *b = (unsigned char *)g->out.p;
+    IncSnap out = inc_snap_at(b, o, true, hc);
+    cudaStream_t st = ctx->stream;
+    if (rows) {
+        CVB_CUDA(ctx, cudaMemcpyAsync(b + i_desc, desc, 64 * rows, cudaMemcpyHostToDevice, st));
+        CVB_CUDA(ctx, cudaMemcpyAsync(b + i_bear, bear, sizeof(double) * 3 * rows, cudaMemcpyHostToDevice, st));
+        if (hc) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_col, col, 3 * rows, cudaMemcpyHostToDevice, st));
+    }
+    if (frames) CVB_CUDA(ctx, cudaMemcpyAsync(b + i_n, n, sizeof(uint32_t) * frames, cudaMemcpyHostToDevice, st));
+    cvb_try_init_result *rd = (cvb_try_init_result *)(b + i_res);
+    if ((rc = try_init_dev(ctx, icfg, tri, arrsac, rngs, better_by, b + i_desc, (const uint32_t *)(b + i_n), (const double *)(b + i_bear),
+                           hc ? b + i_col : nullptr, frames, cap, center, options, F, out.poses, out.vo, out.vl, out.bear, out.desc, out.col, out.lo,
+                           out.obs, out.cons, rd)))
+        return rc;
+    CVB_CUDA(ctx, cudaMemcpyAsync(res, rd, sizeof(cvb_try_init_result), cudaMemcpyDeviceToHost, st));
+    CVB_CUDA(ctx, cvb_wait(ctx, st));
+    if (res->status != CVB_TRY_INIT_CREATED) return 0;
     return inc_download(ctx, out, res->counts, true, hc, poses_out, vo_out, vl_out, bear_out, desc_out, col_out, lo_out, obs_out, cons_out);
 }
 
